@@ -28,6 +28,7 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+HBM_DATASHEET_GBS = 3350.0  # H100 SXM HBM3, NVIDIA data sheet: the roofline's peak when no measured figure is present
 F_DECLARED = {"toy.4p_ssdd_l0.0": 886}  # SURVEY.md §8: frame bytes per replica in the reference's declared dtypes
 
 
@@ -73,7 +74,30 @@ def parse():
                     "1 k / 8 k / 64 k envs per GPU, short runs; the line's top-level keys are the first (headline) entry's")
     ap.add_argument("--matrix-sizes", default="1024,8192,65536")
     ap.add_argument("--skip-extras", action="store_true", help="cim: only the contract keys (value, e2e, roofline, cpu_baseline, clocks)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the decision and metrics rows the timed path returned in its last step as "
+                         "DIR/<name>.npy (float64); inputs are seeded, so two builds can be compared output for output")
     return ap.parse_args()
+
+
+DUMP_BYTES = 64 << 20  # --dump-outputs budget
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each [B, ...] array as out_dir/<name>.npy in float64 (int32 and the int64 metrics are exact there).  Above
+    DUMP_BYTES a fixed, seeded sample of replicas is written instead, with their indices as replica_index.npy."""
+    import numpy as np
+
+    host = {k: (v.cpu().numpy() if hasattr(v, "cpu") else np.asarray(v)).astype(np.float64) for k, v in arrays.items()}
+    B = next(iter(host.values())).shape[0]
+    row_bytes = sum(a[0].nbytes for a in host.values())
+    os.makedirs(out_dir, exist_ok=True)
+    if B * row_bytes > DUMP_BYTES:
+        keep = np.sort(np.random.default_rng(0).choice(B, DUMP_BYTES // row_bytes - 1, replace=False))
+        host = {k: a[keep] for k, a in host.items()}
+        host["replica_index"] = keep.astype(np.float64)
+    for k, a in host.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), a)
 
 
 # ----------------------------------------------------------------------------------------------- clocks
@@ -424,15 +448,15 @@ def cpu_baseline_bike(args, topo):
 
 
 def load_host_agent():
-    """Compile (gcc) and load tools/host_agent.c — the host-side agent of the e2e leg."""
+    """Compile (gcc, into a temporary directory: the source tree may be read-only) and load tools/host_agent.c — the
+    host-side agent of the e2e leg."""
     import ctypes
     import subprocess
+    import tempfile
 
     src = os.path.join(ROOT, "tools", "host_agent.c")
-    out = os.path.join(ROOT, "tools", "_build", "libhost_agent.so")
-    if not os.path.isfile(out) or os.path.getmtime(out) < os.path.getmtime(src):
-        os.makedirs(os.path.dirname(out), exist_ok=True)
-        subprocess.check_call(["gcc", "-O2", "-fopenmp", "-pthread", "-shared", "-fPIC", src, "-o", out])
+    out = os.path.join(tempfile.mkdtemp(prefix="maro_b200_host_agent_"), "libhost_agent.so")
+    subprocess.check_call(["gcc", "-O2", "-fopenmp", "-pthread", "-shared", "-fPIC", src, "-o", out])
     lib = ctypes.CDLL(out)
     lib.agent_random.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32]
     lib.agent_greedy.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -695,6 +719,8 @@ def run_cim(args, rank, local_rank, world):
     total_ms, kernel_ms, launches, _ = primary(args.steps, True)
     wall = time.perf_counter() - wall0
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"decisions": dec, "metrics": met})
     if world > 1:
         dist.barrier()
     c1 = env.counters().sum(0)
@@ -812,7 +838,7 @@ def run_cim(args, rank, local_rank, world):
     line = None
     if rank == 0:
         peaks = _peaks()
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = float(peaks.get("hbm_gbs", HBM_DATASHEET_GBS))
         F = F_DECLARED.get(args.topology, env.frame_words * 4)  # SURVEY.md §8 frame bytes
         n_snap, n_ev = g_snaps / max(1, g_steps), g_events / max(1, g_steps)
         bytes_per_step = 2 * F + n_snap * F + 32 * n_ev + 64
@@ -837,13 +863,13 @@ def run_cim(args, rank, local_rank, world):
                          "bytes_per_env_step": bytes_per_step, "n_snap": n_snap, "n_ev": n_ev,
                          "kernel_us_per_step": 1000.0 * kernel_ms / args.steps,
                          "launch_us": 1000.0 * kernel_ms / max(1, launches),
-                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else "fallback 6650"},
+                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else "H100 SXM data sheet (not reached)"},
             "clocks": clocks, "gpu_launches": launches,
         }
         if e2e:
             line["e2e"] = {"value": g_e2e_steps / (e2e_ms / 1000.0), "unit": "env-steps/s",
-                           # session: one 16-byte command row in, one 64-byte tagged result line out per replica and step
-                           "h2d_bytes_per_step": B * 16, "d2h_bytes_per_step": B * (64 if e2e["n_sub"] else 8 * 4 + 3 * 8),
+                           # session: one 16-byte command row in, one 80-byte tagged result line out per replica and step
+                           "h2d_bytes_per_step": B * 16, "d2h_bytes_per_step": B * (80 if e2e["n_sub"] else 8 * 4 + 3 * 8),
                            "api": ("maro_cim_submit_pinned / maro_cim_wait_pinned (pinned host buffers; resident session) driven by the C "
                                    "host loop tools/host_agent.c:e2e_loop_cim_mt, agent on the host" if e2e["n_sub"] else
                                    "maro_cim_step_pinned (pinned host buffers) + tools/host_agent.c on the host"),
@@ -995,6 +1021,8 @@ def run_ours(args, rank, local_rank, world):
     if not fused:
         total_ms = sum(e[0].elapsed_time(e[2]) for e in events)
         kernel_ms = sum(e[1].elapsed_time(e[2]) for e in events)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"decisions": dec, "metrics": met})
     c1 = env.counters().sum(0)
     d_steps, d_ticks, d_events, d_snaps = (int(x) for x in (c1 - c0))
     if fused:  # the extra legs below drive the per-step path from a fresh episode
@@ -1134,7 +1162,7 @@ def run_ours(args, rank, local_rank, world):
                 peaks = json.load(fp)
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = float(peaks.get("hbm_gbs", HBM_DATASHEET_GBS))
         F = 180 if bike else F_DECLARED.get(args.topology, env.frame_words * 4)  # SURVEY.md §8 frame bytes
         n_snap = g_snaps / max(1, g_steps)
         n_ev = g_events / max(1, g_steps)
@@ -1176,7 +1204,7 @@ def run_ours(args, rank, local_rank, world):
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "traffic": traffic, "kernel": ("vm_rollout_kernel" if fused else "vm_step_kernel") if vm else ("bike_step_kernel" if bike else "cim_step_kernel"), "bytes_per_env_step": bytes_per_step,
                          "n_snap": n_snap, "n_ev": n_ev, "kernel_us": 1000.0 * kernel_ms / args.steps,
-                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else "fallback 6650"},
+                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else "H100 SXM data sheet (not reached)"},
             "clocks": clocks,
             "gpu_launches": launches,
         }
@@ -1232,6 +1260,7 @@ def main():
             for B in sizes:
                 a = copy.copy(args)
                 a.scenario, a.replicas, a.skip_extras, a.graph_chunk = scenario, B, True, 0
+                a.dump_outputs = args.dump_outputs if not entries else ""  # the headline entry's outputs
                 a.topology, a.ticks = "toy.4p_ssdd_l0.0", 1000
                 a.steps = args.steps if B <= 8192 else max(64, args.steps // 4)
                 a.cpu_seconds = min(args.cpu_seconds, 3.0) if B == sizes[0] else 0.0

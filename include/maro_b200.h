@@ -1,5 +1,5 @@
 /*
- * maro_b200.h — C ABI of the B200-native batched discrete-event simulation core.
+ * maro_b200.h — C ABI of the H100-native batched discrete-event simulation core.
  *
  * This is the drop-in boundary (SURVEY.md §8b, seam 3): everything `maro.simulator.Env` /
  * `maro.vector_env.VectorEnv` need from the step path, for B independent replicas at once, as plain

@@ -1,4 +1,4 @@
-"""maro_b200 — B200-native batched discrete-event simulation core behind MARO's Env / VectorEnv surfaces.
+"""maro_b200 — H100-native batched discrete-event simulation core behind MARO's Env / VectorEnv surfaces.
 
     from maro_b200.simulator import Env
     from maro_b200.vector_env import VectorEnv

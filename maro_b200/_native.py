@@ -47,7 +47,7 @@ def lib():
     if not os.path.isfile(LIB_PATH):
         raise NativeLibraryError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  maro_b200 has no CPU fallback.")
+            "(nvcc, sm_90a).  maro_b200 has no CPU fallback.")
     L = C.CDLL(LIB_PATH)
     vp, i32, u32 = C.c_void_p, C.c_int32, C.c_uint32
     L.maro_last_error.restype = C.c_char_p

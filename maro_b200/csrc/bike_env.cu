@@ -212,7 +212,7 @@ int maro_bike_reset(MaroBikeEnv* e, const uint8_t* mask) {
         CK(cudaMemcpyAsync(d_active, e->h_in, e->B, cudaMemcpyHostToDevice, e->stream));
         a.active = d_active;
     }
-    int threads = 128, blocks = std::min((e->B * 32 + threads - 1) / threads, 148 * 16);
+    int threads = 128, blocks = std::min((e->B * 32 + threads - 1) / threads, e->n_sm * 16);
     bike_reset_kernel<<<blocks, threads, 0, e->stream>>>(e->s, a);
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(e->stream));
@@ -263,7 +263,7 @@ int maro_bike_create(const MaroBikeTopology* topo, const MaroCimConfig* cfg, Mar
     e->grid = std::min(ctas_needed, prop.multiProcessorCount * resident);
     {   // the tick chain runs on each group's leader lane: packed groups serialise their leaders, so spread when possible
         const char* sp = getenv("MARO_B200_SPREAD");
-        const bool want_spread = sp ? atoi(sp) != 0 : e->B <= prop.multiProcessorCount * 128;  // measured: +25..45 % up to 16 k
+        const bool want_spread = sp ? atoi(sp) != 0 : e->B <= prop.multiProcessorCount * 128;  // the leader-lane chain gains from a warp of its own
         if (gpw > 1 && want_spread && 256 + (size_t)s.SW * 4 * 4 <= max_smem) {
             e->spread = true;
             e->warps_per_cta = 4;

@@ -1,4 +1,4 @@
-// cim_env.cu — kernels + C ABI (include/maro_b200.h) of the batched CIM discrete-event core for sm_100a.
+// cim_env.cu — kernels + C ABI (include/maro_b200.h) of the batched CIM discrete-event core for sm_90a (H100).
 //
 // Kernels
 //   cim_step_kernel    one warp = one replica.  The replica's state block (frame | control | event queue) is
@@ -10,7 +10,7 @@
 //   cim_policy_kernel  hashed random agent (bench helper).
 //   cim_rl_*_kernel    RL state / action / reward shaping over the snapshot ring.
 // The citi_bike and vm_scheduling scenarios are bike_env.cu / vm_env.cu (same handle layout, env_common.cuh).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -fmad=false -shared -Xcompiler -fPIC
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false -shared -Xcompiler -fPIC
 //   (-fmad=false: CPython never contracts a*b+c; order generation must round like the reference.)
 #include "env_common.cuh"
 #include <time.h>
@@ -164,6 +164,9 @@ __global__ void cim_policy_kernel(const int32_t* __restrict__ dec, int32_t* __re
 enum { RES_ROLLOUT = 0, RES_SESSION = 1 };
 enum { RES_POLICY_NULL = 0, RES_POLICY_RANDOM = 1 };
 enum { RES_CMD_STEP = 0, RES_CMD_EXIT = 1 };
+// result line of the session: MARO_RES_LINE_CHUNKS tagged 16-byte chunks (see "publish" in the session loop)
+#define MARO_RES_LINE_CHUNKS 5
+#define MARO_RES_LINE_WORDS (4 * MARO_RES_LINE_CHUNKS)
 // command row word 1 (flags): bits 0-7 n_actions | bit 8 active | bit 9 bad action | bit 10 Env.reset before the step |
 //                             bits 16-23 command | bit 24 action type of row 0
 struct ResidentArgs {
@@ -174,9 +177,10 @@ struct ResidentArgs {
     int slice_steps;                // RES_ROLLOUT, sliced: > 0 = lane groups pull (replica, slice of `slice_steps` env-steps) work items
     uint32_t* slice_sync;           //   device: {tickets taken, entries appended, entries[B x (n_slices - 1)]}, zeroed before the launch
     const uint32_t* cmd;            // [B][4] command rows (mapped host memory)
-    uint32_t* results;              // mapped host [B][16]: tagged result lines (see "publish" in the session loop)
+    uint32_t* results;              // mapped host [B][MARO_RES_LINE_WORDS]: tagged result lines (see "publish" in the session loop)
     uint32_t poll_ns, wait_ns;      // back-off of the command poll (PCIe) and of the shared-memory relay wait
     uint32_t* seq_state;            // device [B]: last seq each replica has completed (survives launches and resets)
+    int32_t* rows;                  // device [B][16]: each replica's decision + metrics slot between launches of the session
     const uint32_t* heartbeat;      // mapped host word the host bumps while it is inside submit / wait (any thread)
     uint32_t* exit_flag;            // device word: set (to `epoch`) by the first CTA that gives up waiting; every CTA of the launch
     uint32_t epoch;                 //   leaves at its next poll once it is set, so a launch never ends for only SOME of its CTAs
@@ -189,9 +193,8 @@ __device__ __forceinline__ uint4 ld_sys_v4(const uint32_t* p) {
     return v;
 }
 
-// kMinBlocks = 3 caps the kernel at 77 registers (108 uncapped, no spills either way).  Measured (toy.4p, fused rollouts):
-// +12.5 % at 65 536 replicas, +14 % at 32 768, -7 % at 16 384, -1..2 % at <= 8 192 -- so it is chosen per handle (res_dense)
-// once the grid is several waves deep.  Shared memory, not registers, bounds residency here (2 CTAs per SM in both builds).
+// kMinBlocks = 3 caps the kernel's registers (no spills either way).  It helps grids several waves deep and costs at smaller
+// ones (toy.4p, fused rollouts) -- so it is chosen per handle (res_dense) once the grid is several waves deep.  Shared memory, not registers, bounds residency here (2 CTAs per SM in both builds).
 #ifndef MARO_RES_DENSE_BLOCKS
 #define MARO_RES_DENSE_BLOCKS 3
 #endif
@@ -302,8 +305,9 @@ __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __g
         uint32_t expect = ra.seq_state[rep0] + 1u;
         if (threadIdx.x == 0) *seq_s = expect - 1u;
         __syncthreads();  // (threads that left above do not take part in CTA barriers)
-        if (g.lane < 8) dslot[g.lane] = gdec[g.lane];  // rows of inactive replicas keep their previous contents
-        if (g.lane < 3) mslot[g.lane] = gmet[g.lane];
+        // rows of inactive replicas keep their previous contents.  The slot outlives the launch in device memory: when the
+        // kernel comes back up after an idle exit, the host may not have unpacked every result line of the last step yet.
+        for (int i = g.lane; i < 16; i += G) dslot[i] = ra.rows[(int64_t)rep * 16 + i];
         g.sync();
         for (;;) {
             if (gid == 0) {
@@ -375,30 +379,28 @@ __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __g
                 dslot[MARO_DEC_STATUS] = MARO_STATUS_INACTIVE;
             }
             g.sync();
-            // ---- publish: one 64-byte result line per replica in mapped host memory, two 32-byte sectors, each written by ONE
-            // 256-bit store that carries the sequence number in its last word:
-            //     sector 0 = decision words 0..6 | seq        sector 1 = metrics (3 x int64) | decision word 7 | seq
-            // The host takes a line once both tags show the step it is waiting for — no system fence, no separate flag
-            // (a 32-byte aligned store reaches host memory as one write: tag and payload become visible together).
-            if (g.lane < 2) {
-                uint32_t w[8];
-                if (g.lane == 0) {
+            // ---- publish: one 80-byte result line per replica in mapped host memory, five 16-byte chunks, each written by ONE
+            // 128-bit store that carries the sequence number in its last word.  The 14 payload words (decision words 0..7, then
+            // the metrics as 3 x int64 — dslot and mslot are contiguous) go three to a chunk:
+            //     chunk c = payload words 3c, 3c+1, 3c+2 | seq          (word 14 of the payload is padding)
+            // The host takes a line once all five tags show the step it is waiting for — no system fence, no separate flag
+            // (a 16-byte aligned store reaches host memory as one write: tag and payload become visible together).
+            if (g.lane < MARO_RES_LINE_CHUNKS) {
+                const uint32_t* p = reinterpret_cast<const uint32_t*>(dslot);
+                uint32_t w[3];
 #pragma unroll
-                    for (int i = 0; i < 7; i++) w[i] = (uint32_t)dslot[i];
-                } else {
-                    const uint32_t* m32 = reinterpret_cast<const uint32_t*>(mslot);
-#pragma unroll
-                    for (int i = 0; i < 6; i++) w[i] = m32[i];
-                    w[6] = (uint32_t)dslot[7];
+                for (int i = 0; i < 3; i++) {
+                    const int k = 3 * g.lane + i;
+                    w[i] = k < 14 ? p[k] : 0u;
                 }
-                w[7] = expect;
-                asm volatile("st.relaxed.sys.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(ra.results + (int64_t)rep * 16 + g.lane * 8),
-                             "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])
+                asm volatile("st.relaxed.sys.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(ra.results + (int64_t)rep * MARO_RES_LINE_WORDS + g.lane * 4),
+                             "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(expect)
                              : "memory");
             }
             expect++;
         }
         if (g.lane == 0) ra.seq_state[rep] = expect - 1u;
+        for (int i = g.lane; i < 16; i += G) ra.rows[(int64_t)rep * 16 + i] = dslot[i];
     }
     // ---- write back the block + the light-step hint of the per-step kernel
     if (g.lane == 0) snapshot_drain_lane();
@@ -445,7 +447,7 @@ struct MaroCimEnv : EnvCommon {
                                                      // the replica's next command row (or is applied when the session ends)
     uint32_t *h_beat = nullptr, *hd_beat = nullptr;  // heartbeat word, mapped pinned
     uint32_t* d_slice = nullptr;                     // sliced rollouts: ready queue, 2 + B x (kMaxSlices - 1) words
-    int res_per_sm = 0, n_sm = 0, res_slice_steps = -1;       // resident CTAs per SM; steps per slice (-1 = decide per launch, 0 = never)
+    int res_per_sm = 0, res_slice_steps = -1;        // resident CTAs per SM; steps per slice (-1 = decide per launch, 0 = never)
     uint32_t* d_exit = nullptr;                      // exit flag of the resident kernel (device), compared with launch_epoch
     uint32_t launch_epoch = 0;
     int buf_full_cap = 1, buf_empty_cap = 1;         // buffer ticks the event pool was sized for (set_topology re-validation)
@@ -454,8 +456,9 @@ struct MaroCimEnv : EnvCommon {
     std::vector<uint32_t> cta_seq;                   // per CTA: last step completed (the kernel's seq_state mirrors it)
     std::vector<uint8_t> cta_pending;                // per CTA: a step has been sent and not collected yet
     uint32_t *h_cmd = nullptr, *hd_cmd = nullptr;    // [B][4] command rows, mapped pinned
-    uint32_t *h_res = nullptr, *hd_res = nullptr;    // [B][16] tagged result lines, mapped pinned (64-byte aligned)
+    uint32_t *h_res = nullptr, *hd_res = nullptr;    // [B][MARO_RES_LINE_WORDS] tagged result lines, mapped pinned (16-byte aligned chunks)
     uint32_t* d_seq = nullptr;
+    int32_t* d_rows = nullptr;                       // [B][16] decision + metrics slots of the session (ResidentArgs::rows)
     long long idle_cycles = 400000;
     uint32_t poll_ns = 0, wait_ns = 20;
 };
@@ -677,7 +680,7 @@ static int session_launch_locked(MaroCimEnv* e) {
     ResidentArgs ra;
     memset(&ra, 0, sizeof(ra));
     ra.mode = RES_SESSION; ra.spread = e->res_spread;
-    ra.cmd = e->hd_cmd; ra.results = e->hd_res; ra.seq_state = e->d_seq; ra.poll_ns = e->poll_ns; ra.wait_ns = e->wait_ns;
+    ra.cmd = e->hd_cmd; ra.results = e->hd_res; ra.seq_state = e->d_seq; ra.rows = e->d_rows; ra.poll_ns = e->poll_ns; ra.wait_ns = e->wait_ns;
     ra.idle_cycles = e->idle_cycles; ra.heartbeat = e->hd_beat;
     ra.exit_flag = e->d_exit; ra.epoch = ++e->launch_epoch;  // (epochs start at 1; the flag holds 0 or an older epoch)
     CK(launch_resident(e, a, ra, session_geom(e)));
@@ -695,21 +698,22 @@ static int session_wait_ctas(MaroCimEnv* e, int c0, int c1) {
     timespec ts0;
     clock_gettime(CLOCK_MONOTONIC, &ts0);
     int cta = c0, rep = c0 * gpc;
-    // take the result lines in order; a line is complete when both sector tags carry the awaited sequence number
+    // take the result lines in order; a line is complete when every chunk tag carries the awaited sequence number
     auto advance = [&]() {
         while (cta < c1) {
             if (!e->cta_pending[cta]) { cta++; rep = cta * gpc; continue; }
             const uint32_t want = e->cta_seq[cta] + 1u;
             const int end = std::min(B, (cta + 1) * gpc);
             while (rep < end) {
-                const volatile uint32_t* line = e->h_res + (size_t)rep * 16;
-                if (line[7] != want || line[15] != want) return false;
+                const volatile uint32_t* line = e->h_res + (size_t)rep * MARO_RES_LINE_WORDS;
+                for (int c = 0; c < MARO_RES_LINE_CHUNKS; c++)
+                    if (line[4 * c + 3] != want) return false;
                 __atomic_thread_fence(__ATOMIC_ACQUIRE);  // (x86: loads are not reordered; this stops the compiler)
                 const uint32_t* l = const_cast<const uint32_t*>(line);
-                int32_t* d = dec + (size_t)rep * 8;
-                memcpy(d, l, 28);
-                d[7] = (int32_t)l[14];
-                memcpy(met + (size_t)rep * 3, l + 8, 24);
+                uint32_t p[3 * MARO_RES_LINE_CHUNKS];  // payload: decision words 0..7, metrics 3 x int64
+                for (int c = 0; c < MARO_RES_LINE_CHUNKS; c++) memcpy(p + 3 * c, l + 4 * c, 12);
+                memcpy(dec + (size_t)rep * 8, p, 32);
+                memcpy(met + (size_t)rep * 3, p + 8, 24);
                 rep++;
             }
             e->cta_pending[cta] = 0;
@@ -846,13 +850,15 @@ static int create_device_side(MaroCimEnv* e, const MaroCimTopology* topos, int32
     }
     // ---- resident mode: one replica per warp while the batch is small (spread), packed lane groups otherwise
     CK(cudaHostAlloc(&e->h_cmd, (size_t)B * 16, cudaHostAllocMapped));
-    CK(cudaHostAlloc(&e->h_res, (size_t)B * 64, cudaHostAllocMapped));
+    CK(cudaHostAlloc(&e->h_res, (size_t)B * MARO_RES_LINE_WORDS * 4, cudaHostAllocMapped));
     CK(cudaHostGetDevicePointer((void**)&e->hd_cmd, e->h_cmd, 0));
     CK(cudaHostGetDevicePointer((void**)&e->hd_res, e->h_res, 0));
     memset(e->h_cmd, 0, (size_t)B * 16);
-    memset(e->h_res, 0, (size_t)B * 64);
+    memset(e->h_res, 0, (size_t)B * MARO_RES_LINE_WORDS * 4);
     CK(cudaMalloc(&e->d_seq, (size_t)B * 4));
     CK(cudaMemset(e->d_seq, 0, (size_t)B * 4));
+    CK(cudaMalloc(&e->d_rows, (size_t)B * 64));
+    CK(cudaMemset(e->d_rows, 0, (size_t)B * 64));  // (= the zeroed host rows the first session starts from)
     CK(cudaMalloc(&e->d_slice, (2 + (size_t)B * (kMaxSlices - 1)) * 4));
     CK(cudaMalloc(&e->d_exit, 64));
     CK(cudaMemset(e->d_exit, 0, 64));
@@ -864,8 +870,8 @@ static int create_device_side(MaroCimEnv* e, const MaroCimTopology* topos, int32
     const int gpw = 32 / e->lanes;
     const size_t per_group = (size_t)s.SW * 4 + 64 + 16, max_smem = prop.sharedMemPerBlockOptin;  // block + output slot + command row
     // One replica per warp (spread) while every replica can be resident at once, else 32 / lanes replicas per warp (packed).  The
-    // resident kernel holds 16 warps per SM at 108-128 registers: toy.4p rollouts at 3 072 replicas run 13.1 us per batched step
-    // spread (1.3 waves) against 8.8 us packed, at 2 048 (one wave) 7.5 against 8.5.  MARO_B200_RES_SPREAD=0/1 forces a mode.
+    // resident kernel holds fewer warps per SM than the per-step kernel: a spread grid that needs more than one wave is slower than
+    // the packed one, one that fits is faster.  MARO_B200_RES_SPREAD=0/1 forces a mode.
     const char* rs = getenv("MARO_B200_RES_SPREAD");
     e->res_spread = rs ? atoi(rs) != 0 : (B <= nsm * 32);
     e->n_sm = nsm;
@@ -896,9 +902,8 @@ static int create_device_side(MaroCimEnv* e, const MaroCimTopology* topos, int32
             e->res_spread = 0;
             continue;
         }
-        // Rollouts use the session's launch shape.  (Measured: CTAs of 1 / 2 / 8 warps give the same rollout time from 1 024 to
-        // 16 384 replicas and 8 warps are 2-5 % ahead at 65 536 — the kernel is latency bound per warp, not balance bound per
-        // SM.  MARO_B200_ROLL_WARPS forces a CTA size for A/B runs.)
+        // Rollouts use the session's launch shape.  (The CTA size is not a lever: the kernel is latency bound per warp, not
+        // balance bound per SM.  MARO_B200_ROLL_WARPS forces a CTA size for A/B runs.)
         e->roll = session_geom(e);
         if (const char* fw = getenv("MARO_B200_ROLL_WARPS")) {
             const int cw = std::min(w, std::max(1, atoi(fw)));
@@ -913,7 +918,7 @@ static int create_device_side(MaroCimEnv* e, const MaroCimTopology* topos, int32
         e->cta_pending.assign(e->res_grid, 0);
         if (const char* sl = getenv("MARO_B200_RES_SLICE_STEPS")) e->res_slice_steps = atoi(sl);
         const char* se = getenv("MARO_B200_SESSION");
-        e->session_ok = (se ? atoi(se) != 0 : true) && (int64_t)per_sm * nsm >= e->res_grid && !s.joint;  // (64-byte result lines)
+        e->session_ok = (se ? atoi(se) != 0 : true) && (int64_t)per_sm * nsm >= e->res_grid && !s.joint;  // (fixed-size result lines)
         break;
     }
     e->scenario_id = 1;
@@ -941,7 +946,7 @@ int maro_cim_destroy(MaroCimEnv* e) {
     cudaSetDevice(e->device);
     if (e->session_live.load()) session_end(e);
     cudaFree(e->d_tables); cudaFree(e->d_topo); cudaFree(e->d_mt); cudaFree(e->d_light);
-    cudaFree(e->d_seq); cudaFree(e->d_exit); cudaFree(e->d_slice);
+    cudaFree(e->d_seq); cudaFree(e->d_rows); cudaFree(e->d_exit); cudaFree(e->d_slice);
     if (e->h_cmd) cudaFreeHost(e->h_cmd);
     if (e->h_res) cudaFreeHost(e->h_res);
     if (e->h_beat) cudaFreeHost(e->h_beat);
@@ -1008,7 +1013,7 @@ int maro_cim_create(const MaroCimTopology* topos, int32_t n_topos, const MaroCim
     e->grid = std::min(ctas_needed, prop.multiProcessorCount * resident);
     // small batch, sub-warp groups: one replica per warp while the replicas fit the resident warp slots (<= 32 per SM)
     const char* sp = getenv("MARO_B200_SPREAD");
-    const bool want_spread = sp ? atoi(sp) != 0 : e->B <= prop.multiProcessorCount * 32;  // measured crossover 4 k .. 8 k replicas
+    const bool want_spread = sp ? atoi(sp) != 0 : e->B <= prop.multiProcessorCount * 32;  // every replica gets a resident warp
     if (gpw > 1 && want_spread && 256 + (size_t)s.SW * 4 * 4 <= max_smem) {
         e->spread = true;
         e->warps_per_cta = 4;
@@ -1067,7 +1072,7 @@ static int reset_now(MaroCimEnv* e, const uint8_t* mask) {
     } else {
         std::fill(e->reset_pending.begin(), e->reset_pending.end(), (uint8_t)0);
     }
-    int threads = 128, blocks = std::min((e->B * 32 + threads - 1) / threads, 148 * 16);
+    int threads = 128, blocks = std::min((e->B * 32 + threads - 1) / threads, e->n_sm * 16);
     cim_reset_kernel<<<blocks, threads, 0, e->stream>>>(e->s, a);
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(e->stream));
@@ -1237,9 +1242,7 @@ int maro_cim_rollout_device(MaroCimEnv* e, int32_t policy, uint32_t seed, uint32
     ResGeom geo = e->roll;
     const int capacity = geo.per_sm * e->n_sm;
     int slice_steps = 0;
-    // (one replica per warp only: lane groups that share a warp would serialise once they run different slices.  Measured on
-    // BASELINE config #4, 1 024 replicas = 171 CTAs on 148 SMs: 46.0 -> 32.4 us per batched env-step; 4 / 8 / 16 steps per slice
-    // within 3 % of each other)
+    // (one replica per warp only: lane groups that share a warp would serialise once they run different slices)
     const bool warp_per_replica = e->res_spread || e->lanes == 32;
     if (e->res_slice_steps > 0) slice_steps = e->res_slice_steps;  // (forced: tests, A/B)
     else if (e->res_slice_steps < 0 && capacity > 0 && geo.grid > capacity && n_steps >= 16) {
@@ -1348,7 +1351,7 @@ static int rl_state_launch(MaroCimEnv* e, const int32_t* d_decisions, int32_t lo
     q.decisions = d_decisions; q.look_back_ticks = look_back - 1; q.n_ports_per_state = 1 + e->s.fut;
     q.npa = n_port_attrs; q.nva = n_vessel_attrs; q.state_out = d_out; q.state_out_f32 = d_out_f32;
     const int64_t total = (int64_t)e->B * maro_cim_rl_state_dim(e, look_back, n_port_attrs, n_vessel_attrs);
-    int threads = 256, blocks = (int)std::min<int64_t>((total + threads - 1) / threads, 148 * 8);
+    int threads = 256, blocks = (int)std::min<int64_t>((total + threads - 1) / threads, (int64_t)e->n_sm * 8);
     cim_rl_state_kernel<<<blocks, threads, 0, e->stream>>>(q);
     CK(cudaGetLastError());
     return 0;
@@ -1416,7 +1419,7 @@ static int rl_reward_launch(MaroCimEnv* e, const int32_t* d_ticks, const int32_t
     q.off_shortage = e->attrs[0][common_attr_id(e, 0, "shortage")].off;
     q.fulfillment_factor = fulfillment_factor; q.shortage_factor = shortage_factor; q.reward_out = d_out;
     const int64_t items = (int64_t)n_rows * e->B;
-    int threads = 128, blocks = (int)std::min<int64_t>((items * 32 + threads - 1) / threads, 148 * 16);
+    int threads = 128, blocks = (int)std::min<int64_t>((items * 32 + threads - 1) / threads, (int64_t)e->n_sm * 16);
     cim_rl_reward_kernel<<<blocks, threads, 0, e->stream>>>(q);
     CK(cudaGetLastError());
     return 0;

@@ -123,6 +123,7 @@ struct AttrInfo { const char* name; int off, slots, isf, n_nodes; };
 // query scratch, attribute registry.
 struct EnvCommon {
     int device = 0, B = 0;
+    int n_sm = 1;  // SMs of the device (grid size of the grid-stride kernels)
     int ring_rows = 0, FW = 0, FWp = 0, SW = 0;
     int off_tick = 0, off_counters = 0;  // word offsets inside a replica's state block
     int dec_words = 8, max_actions = 1, met_words = 3;  // decision row int32 words, metrics row int64 words
@@ -161,6 +162,7 @@ static void common_free(EnvCommon* e) {
 static int common_alloc(EnvCommon* e) {
     CK(cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking));
     e->stream = e->own_stream;
+    CK(cudaDeviceGetAttribute(&e->n_sm, cudaDevAttrMultiProcessorCount, e->device));
     const size_t B = (size_t)e->B;
     CK(cudaMalloc(&e->d_state, B * e->SW * 4));
     CK(cudaMalloc(&e->d_snap, B * e->ring_rows * e->FWp * 4));
@@ -411,7 +413,7 @@ static int query_impl(EnvCommon* e, const int32_t* replicas, int32_t nr, int32_t
     q.layout = e->query_layout; q.max_slots = max_slots;
     q.out = dst;
     int threads = 256;
-    int blocks = (int)std::min<int64_t>((total + threads - 1) / threads, 148 * 8);
+    int blocks = (int)std::min<int64_t>((total + threads - 1) / threads, (int64_t)e->n_sm * 8);
     cim_query_kernel<<<blocks, threads, 0, e->stream>>>(q);
     CK(cudaGetLastError());
     if (h_out) CK(cudaMemcpyAsync(h_out, dst, (size_t)total * 8, cudaMemcpyDeviceToHost, e->stream));

@@ -184,7 +184,7 @@ static int vm_reset_impl(MaroVmEnv* e, const uint8_t* mask, int init_ring) {
         CK(cudaMemcpyAsync(d_active, e->h_in, e->B, cudaMemcpyHostToDevice, e->stream));
         a.active = d_active;
     }
-    int threads = 128, blocks = std::min((e->B * 32 + threads - 1) / threads, 148 * 16);
+    int threads = 128, blocks = std::min((e->B * 32 + threads - 1) / threads, e->n_sm * 16);
     vm_reset_kernel<<<blocks, threads, 0, e->stream>>>(e->s, a, init_ring);
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(e->stream));
@@ -324,7 +324,7 @@ int maro_vm_rollout_device(MaroVmEnv* e, int32_t n_steps, int32_t* d_decisions, 
 int maro_vm_best_fit_policy_device(MaroVmEnv* e, const int32_t* d_decisions, int32_t* d_actions) {
     if (!e || !d_decisions || !d_actions) return fail("maro_vm_best_fit_policy_device: bad arguments");
     CK(cudaSetDevice(e->device));
-    int threads = 128, blocks = std::min((e->B * 32 + threads - 1) / threads, 148 * 16);
+    int threads = 128, blocks = std::min((e->B * 32 + threads - 1) / threads, e->n_sm * 16);
     vm_best_fit_kernel<<<blocks, threads, 0, e->stream>>>(e->s, e->d_state, d_decisions, d_actions);
     CK(cudaGetLastError());
     return 0;

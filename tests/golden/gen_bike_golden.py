@@ -139,6 +139,15 @@ def prepare_reference_cases():
             conf = yaml.safe_load(fp)
         with open(os.path.join(dst, "decision.yml"), "w") as fp:
             yaml.safe_dump({"decision": conf["decision"], "time_zone": conf["time_zone"]}, fp, sort_keys=False)
+    # the reference's data_lib test metas (tests/data/data_lib/case_{1,2}/meta.yml, kept as tests/golden/data_lib/trips_tz*.meta.yml)
+    # on their trips.csv (= tests/golden/data_lib/trips_case_1.csv): byte-identity cases of tests/test_data_lib.py
+    dl = os.path.join(HERE, "data_lib")
+    for meta, out in (("trips_tz_events.meta.yml", "trips_case_1_tz_events.bin"), ("trips_tz.meta.yml", "trips_case_1_tz.bin")):
+        if not os.path.isfile(os.path.join(dl, out)):
+            conv = BinaryConverter(os.path.join(dl, out), os.path.join(dl, meta))
+            conv.add_csv(os.path.join(dl, "trips_case_1.csv"))
+            conv.flush()
+            del conv
 
 
 def run_case(name, spec, out_dir=None):

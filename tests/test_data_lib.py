@@ -1,6 +1,6 @@
 """CPU: maro_b200.data_lib.BinaryConverter (SURVEY.md §8f rank 3) against the reference's own csv / bin fixture pairs
-(reference tests/data/citi_bike, tests/data/vm_scheduling — the .bin files were written by the reference's converter:
-either shipped next to the csv in its test data, or converted here by tests/golden/gen_bike_golden.py) — byte for byte —
+(reference tests/data/citi_bike, tests/data/vm_scheduling, tests/data/data_lib — the .bin files were written by the reference's
+converter: either shipped next to the csv in its test data, or converted here by tests/golden/gen_bike_golden.py) — byte for byte —
 and the round trip through the reader the scenario loaders use."""
 import os
 
@@ -13,19 +13,25 @@ G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 D = os.path.join(G, "data_lib")
 
 PAIRS = [
-    # csv, meta, reference-written bin
-    ("trips_case_1.csv", "trips.meta.yml", os.path.join(G, "bike_case_1", "trips.bin")),
-    ("trips_case_2.csv", "trips.meta.yml", os.path.join(G, "bike_case_2", "trips.bin")),
-    ("weather.csv", "weather.meta.yml", os.path.join(G, "bike_case_1", "weathers.bin")),
-    ("vmtable_toy.csv", "vmtable_toy.meta.yml", os.path.join(G, "vm_toy", "vmtable_toy.bin")),
-    ("vm_cpu_readings-file-1-of-toy.csv", "cpu_readings.yml", os.path.join(G, "vm_toy", "vm_cpu_readings-file-1-of-toy.bin")),
-    ("vmtable_test.csv", "vmtable.meta.yml", os.path.join(D, "vmtable_test.bin")),
-    ("vm_cpu_readings-file-2-of-test.csv", "cpu_readings.yml", os.path.join(D, "vm_cpu_readings-file-2-of-test.bin")),
+    # csv, meta, reference-written bin (relative to tests/golden: test ids must not depend on where the checkout lives)
+    ("trips_case_1.csv", "trips.meta.yml", "bike_case_1/trips.bin"),
+    ("trips_case_2.csv", "trips.meta.yml", "bike_case_2/trips.bin"),
+    ("weather.csv", "weather.meta.yml", "bike_case_1/weathers.bin"),
+    ("vmtable_toy.csv", "vmtable_toy.meta.yml", "vm_toy/vmtable_toy.bin"),
+    ("vm_cpu_readings-file-1-of-toy.csv", "cpu_readings.yml", "vm_toy/vm_cpu_readings-file-1-of-toy.bin"),
+    ("vmtable_test.csv", "vmtable.meta.yml", "data_lib/vmtable_test.bin"),
+    ("vm_cpu_readings-file-2-of-test.csv", "cpu_readings.yml", "data_lib/vm_cpu_readings-file-2-of-test.bin"),
+    ("vm_cpu_readings-file-1-of-test.csv", "cpu_readings.yml", "data_lib/vm_cpu_readings-file-1-of-test.bin"),
+    ("vm_cpu_readings-file-3-of-test.csv", "cpu_readings.yml", "data_lib/vm_cpu_readings-file-3-of-test.bin"),
+    # the reference's data_lib metas: a source time zone to convert from (dropped by its converter), with / without events
+    ("trips_case_1.csv", "trips_tz_events.meta.yml", "data_lib/trips_case_1_tz_events.bin"),
+    ("trips_case_1.csv", "trips_tz.meta.yml", "data_lib/trips_case_1_tz.bin"),
 ]
 
 
 @pytest.mark.parametrize("csv_name,meta_name,ref_bin", PAIRS)
 def test_converter_output_is_byte_identical_to_the_reference(tmp_path, csv_name, meta_name, ref_bin):
+    ref_bin = os.path.join(G, *ref_bin.split("/"))
     out = str(tmp_path / "out.bin")
     conv = BinaryConverter(out, os.path.join(D, meta_name))
     conv.add_csv(os.path.join(D, csv_name))

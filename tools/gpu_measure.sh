@@ -1,5 +1,5 @@
 #!/bin/bash
-# Round-end measurement session on one B200: default bench line, the north-star matrix, the secondary workloads.
+# Round-end measurement session on one H100: default bench line, the north-star matrix, the secondary workloads.
 tag=${1:-r2}
 mkdir -p gpurun_out
 cp maro_b200/libmaro_b200.so gpurun_out/${tag}_lib.so

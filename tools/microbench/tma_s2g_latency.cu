@@ -1,6 +1,6 @@
 // Microbenchmark: latency of one cp.async.bulk shared -> global store of N bytes until the source may be reused
 // (wait_group.read) and until the write is complete (wait_group), vs a lane-group copy with 128-bit stores.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 tma_s2g_latency.cu -o tma_s2g_latency
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 tma_s2g_latency.cu -o tma_s2g_latency
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
