@@ -160,6 +160,10 @@ __device__ __forceinline__ int maro_clz(uint32_t x) { return __clz((int)x); }
 #define LANE_DIM(i, n) for (int i = g.lane; i < (n); i += (G < 32 ? 0x40000000 : G))
 #endif
 
+// chunks of G over a topology dimension that every lane group of the small-topology instantiation covers in one pass
+// (kSmall: P, V, route lengths and fut are <= G): a constant trip count of one there
+#define GROUP_CHUNKS(b0, n) for (int b0 = 0; b0 < (kSmall ? 1 : (n)); b0 += G)
+
 // inclusive prefix sum over the lanes of a group
 template <int G>
 MARO_DEV int scan_incl(const Grp<G>& g, int x) {
@@ -235,6 +239,32 @@ struct CimShape {
     int joint, DW;
 };
 
+// ---------------------------------------------------------------------------------------------------
+// Per-phase cycle attribution of the step's dependent chain, compiled in only with -DMARO_PHASE_CLOCKS (tools/phase_clocks.py
+// builds that variant).  PHASE_MARK(r, ph) charges the cycles since the previous mark to phase `ph`; the resident rollout keeps
+// the accumulators in registers and adds them to maro_phase_clk once per launch.
+// ---------------------------------------------------------------------------------------------------
+enum Phase { PH_AGENT, PH_ACTIONS, PH_VESSELS, PH_BUCKET, PH_DELAY, PH_ORDERS, PH_ARRIVALS, PH_DECISION, PH_POST, PH_STORE,
+             PH_COUNT, PH_STEPS = PH_COUNT, PH_TICKS, PH_SLOTS };
+#if defined(MARO_PHASE_CLOCKS) && !defined(MARO_HOST_EMULATION)
+struct PhaseClk {
+    long long t;                   // clock64() at the previous mark
+    unsigned long long acc[PH_SLOTS];  // cycles per phase, then env-steps and ticks
+};
+#define PHASE_MARK(r, ph)                              \
+    do {                                               \
+        if ((r).pc) {                                  \
+            const long long _t = clock64();            \
+            (r).pc->acc[ph] += (unsigned long long)(_t - (r).pc->t); \
+            (r).pc->t = _t;                            \
+        }                                              \
+    } while (0)
+#define PHASE_COUNT(r, slot, n) do { if ((r).pc) (r).pc->acc[slot] += (unsigned long long)(n); } while (0)
+#else
+#define PHASE_MARK(r, ph) do {} while (0)
+#define PHASE_COUNT(r, slot, n) do {} while (0)
+#endif
+
 struct Replica {
     int32_t* f;          // frame words (shared memory on the device)
     int32_t* c;          // control words
@@ -243,6 +273,9 @@ struct Replica {
     uint32_t* mt;        // [2][640] MT19937 states + scratch, global memory (NULL when the topology has no noise)
     int32_t* snap;       // [ring_rows][FWp] snapshot ring (global)
     int32_t* snap_frame; // [ring_rows] frame index held by each row
+#if defined(MARO_PHASE_CLOCKS) && !defined(MARO_HOST_EMULATION)
+    PhaseClk* pc;        // phase accumulators of this lane (resident rollouts only, else NULL)
+#endif
 };
 
 #define TBL_I(r, off, i) ((r).t[(off) + (i)])
@@ -255,6 +288,67 @@ MARO_DEV int32_t& VA(const CimShape& s, const Replica& r, int attr, int v) { ret
 MARO_DEV int64_t ctrl_get64(const Replica& r, int lo) { return *reinterpret_cast<const int64_t*>(r.c + lo); }
 MARO_DEV void ctrl_set64(const Replica& r, int lo, int64_t v) { *reinterpret_cast<int64_t*>(r.c + lo) = v; }
 MARO_DEV void ctrl_add64(const Replica& r, int lo, int64_t d) { ctrl_set64(r, lo, ctrl_get64(r, lo) + d); }
+
+// ------------------------------------------------------------------------------------------------
+// Control state that replica_step reads or writes on every step, held in registers for as long as the block stays on the SM
+// (a resident launch: loaded once after stage-in, stored once before write-back; other callers around each call).  The
+// scalars are the same in every lane of the group; the 64-bit counters are kept by the leader lane.  In the small-topology
+// instantiation (kSmall: V <= G) lane v also holds vessel v's three cursors C_FIXED + {0, V, 2V} + v.  What stays in the
+// control block (free stack top, error word, MT19937 positions, ...) is shared-memory state of the phases that use it.
+// ------------------------------------------------------------------------------------------------
+struct Ctl {
+    int state, tick, dec_pos, ep_step, last_frame;
+    uint64_t arr;  // vessels arriving this tick (C_ARR_LO / C_ARR_HI)
+    int64_t opnum, nsteps, nticks, nevents, nsnaps;
+    int dep_cursor, next_dep, next_arr;  // kSmall: vessel g.lane's cursors (NO_TICK on lanes >= V)
+};
+
+template <int G, bool kSmall>
+MARO_DEV void ctl_load(const CimShape& s, const Grp<G>& g, const Replica& r, Ctl& k) {
+    k.state = r.c[C_STATE];
+    k.tick = r.c[C_TICK];
+    k.dec_pos = r.c[C_DEC_POS];
+    k.ep_step = r.c[C_EP_STEP];
+    k.last_frame = r.c[C_LAST_FRAME];
+    k.arr = ((uint64_t)(uint32_t)r.c[C_ARR_HI] << 32) | (uint32_t)r.c[C_ARR_LO];
+    k.opnum = ctrl_get64(r, C_OPNUM_LO);
+    k.nsteps = ctrl_get64(r, C_NSTEPS_LO);
+    k.nticks = ctrl_get64(r, C_NTICKS_LO);
+    k.nevents = ctrl_get64(r, C_NEVENTS_LO);
+    k.nsnaps = ctrl_get64(r, C_NSNAPS_LO);
+    const int v = g.lane;
+    const bool in = kSmall && v < s.V;
+    k.dep_cursor = in ? r.c[C_FIXED + v] : 0;
+    k.next_dep = in ? r.c[C_FIXED + s.V + v] : NO_TICK;
+    k.next_arr = in ? r.c[C_FIXED + 2 * s.V + v] : NO_TICK;
+}
+
+// (ends with a group barrier: the control block is complete for every lane afterwards)
+template <int G, bool kSmall>
+MARO_DEV void ctl_store(const CimShape& s, const Grp<G>& g, const Replica& r, const Ctl& k) {
+    g.sync();
+    if (g.lane == 0) {
+        r.c[C_STATE] = k.state;
+        r.c[C_TICK] = k.tick;
+        r.c[C_DEC_POS] = k.dec_pos;
+        r.c[C_EP_STEP] = k.ep_step;
+        r.c[C_LAST_FRAME] = k.last_frame;
+        r.c[C_ARR_LO] = (int32_t)(uint32_t)(k.arr & 0xffffffffu);
+        r.c[C_ARR_HI] = (int32_t)(uint32_t)(k.arr >> 32);
+        ctrl_set64(r, C_OPNUM_LO, k.opnum);
+        ctrl_set64(r, C_NSTEPS_LO, k.nsteps);
+        ctrl_set64(r, C_NTICKS_LO, k.nticks);
+        ctrl_set64(r, C_NEVENTS_LO, k.nevents);
+        ctrl_set64(r, C_NSNAPS_LO, k.nsnaps);
+    }
+    const int v = g.lane;
+    if (kSmall && v < s.V) {
+        r.c[C_FIXED + v] = k.dep_cursor;
+        r.c[C_FIXED + s.V + v] = k.next_dep;
+        r.c[C_FIXED + 2 * s.V + v] = k.next_arr;
+    }
+    g.sync();
+}
 
 // ------------------------------------------------------------------------------------------------
 // MT19937, bit-compatible with CPython's random.Random (Modules/_randommodule.c).
@@ -364,13 +458,40 @@ MARO_DEV uint16_t* q_free(const CimShape& s, const Replica& r) { return q_next(s
 MARO_DEV int32_t* dl_slot(const CimShape& s, const Replica& r, int tick) { return r.f + s.o_dl + (tick & (s.DL - 1)) * s.dl_stride; }
 
 // Drain the delay-line slot of `tick`: every accumulated RETURN_FULL (:499-522) and RETURN_EMPTY (:695-706) of this tick.
-template <int G>
+// kSmall (P <= G): lane p drains source port p's row and port p's RETURN_EMPTY entry, then applies the row's total to port p
+// -- the same integer sums with plain updates of the lane's own port instead of shared-memory atomics on shared ports.
+template <int G, bool kSmall>
 MARO_DEV int run_delay_line(const CimShape& s, const Grp<G>& g, const Replica& r, int tick) {
     int32_t* sl = dl_slot(s, r, tick);
     const int PP = s.P * s.P;
     const int n = sl[PP + s.P] + sl[PP + s.P + 1];
     if (n == 0) return 0;  // group-uniform
     g.sync();
+    if (kSmall) {
+        const int p = g.lane;
+        if (p < s.P) {
+            int32_t* row = sl + p * s.P;
+            int32_t* fop = r.f + s.o_fop + p * s.P;
+            int tot = 0;
+            for (int d = 0; d < s.P; d++) {
+                const int q = row[d];
+                if (q) { fop[d] += q; row[d] = 0; tot += q; }
+            }
+            if (tot) {
+                PA(s, r, PA_ON_SHIPPER, p) -= tot;
+                PA(s, r, PA_FULL, p) += tot;
+            }
+            const int qe = sl[PP + p];
+            if (qe) {
+                PA(s, r, PA_ON_CONSIGNEE, p) -= qe;
+                PA(s, r, PA_EMPTY, p) += qe;
+                sl[PP + p] = 0;
+            }
+        }
+        if (g.lane == 0) { sl[PP + s.P] = 0; sl[PP + s.P + 1] = 0; }  // (every lane read them above the barrier)
+        g.sync();
+        return n;
+    }
     int src = g.lane / s.P, dst = g.lane - src * s.P;
     for (int i = g.lane; i < PP; i += G) {
         const int q = sl[i];
@@ -455,9 +576,12 @@ MARO_DEV void group_push(const CimShape& s, const Grp<G>& g, const Replica& r, b
 // Static-table helpers (maro/data_lib/cim/vessel_*_wrapper.py, vessel_future_stops_prediction.py)
 // ------------------------------------------------------------------------------------------------
 // Vessel._update_remaining_space (vessel.py:113-120); total_space = floor(capacity / container_volume)
-MARO_DEV int total_space(const CimShape& s, int cap) { return s.vol_is_one ? cap : (int)maro_floor((double)cap / s.vol); }
+// (kSmall: container volume 1)
+template <bool kSmall = false>
+MARO_DEV int total_space(const CimShape& s, int cap) { return kSmall || s.vol_is_one ? cap : (int)maro_floor((double)cap / s.vol); }
+template <bool kSmall = false>
 MARO_DEV void vessel_update_space(const CimShape& s, const Replica& r, int v) {
-    VA(s, r, VA_REMAINING_SPACE, v) = total_space(s, VA(s, r, VA_CAPACITY, v)) - VA(s, r, VA_FULL, v) - VA(s, r, VA_EMPTY, v);
+    VA(s, r, VA_REMAINING_SPACE, v) = total_space<kSmall>(s, VA(s, r, VA_CAPACITY, v)) - VA(s, r, VA_FULL, v) - VA(s, r, VA_EMPTY, v);
 }
 
 // VesselPastStopsWrapper.__getitem__ (:23-38) + Vessel.set_stop_list (vessel.py:91-111) — one lane per vessel
@@ -507,7 +631,7 @@ MARO_DEV void predict_serial(const CimShape& s, const Replica& r, int v, int sto
 // Phase (b): events queued for this tick by earlier ticks.  _on_full_return (:499-522), _on_empty_return (:695-706),
 // _on_discharge (:658-693) are pure adds -> shared-memory atomics in any order; RETURN_EMPTY pushes keep lane order.
 // ------------------------------------------------------------------------------------------------
-template <int G, bool kGeneral>
+template <int G, bool kGeneral, bool kSmall>
 MARO_DEV int run_bucket(const CimShape& s, const Grp<G>& g, const Replica& r, int tick) {
     int32_t* bk = q_bucket(s, r) + (tick & (s.QH - 1));
     int head = *bk & 0xffff;
@@ -574,7 +698,7 @@ MARO_DEV int run_bucket(const CimShape& s, const Grp<G>& g, const Replica& r, in
         if (g.lane == 0) { r.c[C_FREE_TOP] = top + n; r.c[C_Q_COUNT] -= n; }
         g.sync();
         if (db) {
-            if (!kGeneral && s.DL) {
+            if (!kGeneral && (kSmall || s.DL)) {
                 if (is_dis && buf > 0 && tick + buf < s.max_tick) {
                     int32_t* sl = dl_slot(s, r, tick + buf);
                     atomic_add(&sl[s.P * s.P + c], qty);
@@ -596,7 +720,7 @@ MARO_DEV int run_bucket(const CimShape& s, const Grp<G>& g, const Replica& r, in
 // orders of one source port consume `empty` in sequence -> segmented prefix sum (orders arrive sorted by source).
 // `get(i, w, q)` yields order i as {src | dst << 8, qty}.
 // ------------------------------------------------------------------------------------------------
-template <int G, bool kGeneral, class Get>
+template <int G, bool kGeneral, bool kSmall, class Get>
 MARO_DEV int run_orders(const CimShape& s, const Grp<G>& g, const Replica& r, int tick, int n_orders, Get get) {
     int nev = 0;
     for (int base = 0; base < n_orders; base += G) {
@@ -644,7 +768,7 @@ MARO_DEV int run_orders(const CimShape& s, const Grp<G>& g, const Replica& r, in
             atomic_add(&r.f[s.o_fop + src * s.P + dst], exec);
         }
         nev += nv + maro_popc(g.ballot(imm));
-        if (!kGeneral && s.DL) {
+        if (!kGeneral && (kSmall || s.DL)) {
             if (valid && buf > 0 && tick + buf < s.max_tick) {
                 int32_t* sl = dl_slot(s, r, tick + buf);
                 atomic_add(&sl[src * s.P + dst], exec);
@@ -837,7 +961,7 @@ MARO_DEV int gen_orders_coop(const CimShape& s, const Grp<G>& g, const Replica& 
 // ------------------------------------------------------------------------------------------------
 // Phase (d): VESSEL_ARRIVAL (:600-632) + LOAD_FULL (:524-598) of one arriving vessel, lanes over route positions.
 // ------------------------------------------------------------------------------------------------
-template <int G>
+template <int G, bool kSmall>
 MARO_DEV void run_arrival(const CimShape& s, const Grp<G>& g, const Replica& r, int tick, int v) {
     const int loc = VA(s, r, VA_NEXT_LOC_IDX, v);
     const int sb = TBL_I(r, s.t_stop_offset, v);
@@ -852,7 +976,7 @@ MARO_DEV void run_arrival(const CimShape& s, const Grp<G>& g, const Replica& r, 
         int pos0 = (TBL_I(r, s.t_vessel_route_start, v) + loc) % rl;
         int arrival0 = TBL_I(r, s.t_stop_arrival, sb + loc);
         int n = rl > s.fut ? rl : s.fut;
-        for (int b0 = 0; b0 < n; b0 += G) {  // n <= G in every shipped topology; loop keeps it general
+        GROUP_CHUNKS(b0, n) {  // n <= G in every shipped topology; loop keeps it general
             int k = b0 + g.lane;
             int pos = pos0 + k;  // pos0 < rl and k < max(rl, fut): a few conditional subtractions instead of a division
             while (pos >= rl) pos -= rl;
@@ -871,11 +995,11 @@ MARO_DEV void run_arrival(const CimShape& s, const Grp<G>& g, const Replica& r, 
     // ---- _on_full_load
     const int cap = VA(s, r, VA_CAPACITY, v);
     int full = VA(s, r, VA_FULL, v);
-    int acceptable = s.vol_is_one ? cap - full : (int)maro_floor(((double)cap - (double)full * s.vol) / s.vol);
+    int acceptable = kSmall || s.vol_is_one ? cap - full : (int)maro_floor(((double)cap - (double)full * s.vol) / s.vol);
     if (acceptable < 0) acceptable = 0;
     int total_loaded = 0;
     g.sync();
-    for (int b0 = 0; b0 < rl; b0 += G) {  // reachable stops: stops[loc + 1 : loc + 1 + route_len]
+    GROUP_CHUNKS(b0, rl) {  // reachable stops: stops[loc + 1 : loc + 1 + route_len]
         int k = b0 + g.lane;
         int si = loc + 1 + k;
         bool valid = k < rl && si < ns;
@@ -910,15 +1034,16 @@ MARO_DEV void run_arrival(const CimShape& s, const Grp<G>& g, const Replica& r, 
         int empty = VA(s, r, VA_EMPTY, v);
         int total_container = full + empty;
         int early = 0;
-        bool over = s.vol_is_one ? total_container > cap : (double)total_container * s.vol > (double)cap;
+        const bool vol1 = kSmall || s.vol_is_one;
+        bool over = vol1 ? total_container > cap : (double)total_container * s.vol > (double)cap;
         if (over) {
-            early = total_container - (s.vol_is_one ? cap : (int)maro_ceil((double)cap / s.vol));
+            early = total_container - (vol1 ? cap : (int)maro_ceil((double)cap / s.vol));
             empty -= early;
             VA(s, r, VA_EMPTY, v) = empty;
             PA(s, r, PA_EMPTY, port) += early;
         }
         VA(s, r, VA_EARLY_DISCHARGE, v) = early;
-        VA(s, r, VA_REMAINING_SPACE, v) = total_space(s, cap) - full - empty;
+        VA(s, r, VA_REMAINING_SPACE, v) = total_space<kSmall>(s, cap) - full - empty;
     }
     g.sync();
 }
@@ -936,8 +1061,8 @@ struct Act4 { int32_t v, p, qty, type; };
 
 // _on_action_received (:708-748).  Lane k holds action k (loaded with one 128-bit read); the leader lane applies them in
 // order.  Returns false where the reference would raise AssertionError.
-template <int G>
-MARO_DEV bool on_actions(const CimShape& s, const Grp<G>& g, const Replica& r, const Act4& mine, int n) {
+template <int G, bool kSmall>
+MARO_DEV bool on_actions(const CimShape& s, const Grp<G>& g, const Replica& r, Ctl& k, const Act4& mine, int n) {
     bool ok = true;
     for (int i = 0; i < n; i++) {
         int v = g.shfl(mine.v, i), p = g.shfl(mine.p, i), move = g.shfl(mine.qty, i), type = g.shfl(mine.type, i);
@@ -955,8 +1080,8 @@ MARO_DEV bool on_actions(const CimShape& s, const Grp<G>& g, const Replica& r, c
             PA(s, r, PA_EMPTY, p) = port_empty - move;
             VA(s, r, VA_EMPTY, v) = vessel_empty + move;
         }
-        vessel_update_space(s, r, v);
-        ctrl_add64(r, C_OPNUM_LO, move);
+        vessel_update_space<kSmall>(s, r, v);
+        k.opnum += move;  // (leader lane)
         // port.transfer_cost (float32 attr) += move: python float (double) add, stored back as float32
         float tc = maro_i2f(PA(s, r, PA_TRANSFER_COST, p));
         PA(s, r, PA_TRANSFER_COST, p) = maro_f2i(maro_d2f((double)tc + (double)move));
@@ -987,7 +1112,7 @@ MARO_DEV void snapshot_wait(const Grp<G>& g) {
 }
 
 template <int G>
-MARO_DEV void take_snapshot(const CimShape& s, const Grp<G>& g, const Replica& r, int frame_index) {
+MARO_DEV void take_snapshot(const CimShape& s, const Grp<G>& g, const Replica& r, Ctl& k, int frame_index) {
     int row = frame_index < s.ring_rows ? frame_index : frame_index % s.ring_rows;
     int32_t* dst = r.snap + (int64_t)row * s.FWp;
 #ifdef MARO_HOST_EMULATION
@@ -1007,11 +1132,9 @@ MARO_DEV void take_snapshot(const CimShape& s, const Grp<G>& g, const Replica& r
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     }
 #endif
-    if (g.lane == 0) {
-        r.snap_frame[row] = frame_index;
-        r.c[C_LAST_FRAME] = frame_index;
-        ctrl_add64(r, C_NSNAPS_LO, 1);
-    }
+    if (g.lane == 0) r.snap_frame[row] = frame_index;
+    k.last_frame = frame_index;
+    k.nsnaps += 1;
 }
 
 // Output rows are written with 128-bit / 64-bit stores (they may live in mapped host memory: one PCIe write each).
@@ -1025,8 +1148,9 @@ MARO_DEV void store_out(int32_t* dec, int64_t* met, const int32_t* od, int64_t m
     met[0] = m0; met[1] = m1; met[2] = m2;
 }
 
+template <bool kSmall = false>
 MARO_DEV int frame_index_of(const CimShape& s, int tick) {
-    return s.res_is_one ? tick - s.start_tick : (tick - s.start_tick) / s.resolution;
+    return kSmall || s.res_is_one ? tick - s.start_tick : (tick - s.start_tick) / s.resolution;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1034,15 +1158,22 @@ MARO_DEV int frame_index_of(const CimShape& s, int tick) {
 // (3 int64) its output rows.  All lanes of the group call this together.
 // ------------------------------------------------------------------------------------------------
 // kGeneral = false compiles the noise-free fast path only (static order schedule, integer buffer ticks, no MT19937).
-template <int G, bool kGeneral>
-MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r, const Act4& act, int n_act,
+// kSmall (with kGeneral = false) compiles the small-topology path: resolution 1, container volume 1, Sequential mode, delay
+// lines on, and P, V, route lengths and fut <= G (cim_small_ok) -- every lane loop over them is one pass, the vessel cursors
+// live in Ctl.  Sizes and table offsets stay runtime values.
+// The control state is `k` (ctl_load before, ctl_store after: the control block in shared memory is stale in between).
+template <int G, bool kGeneral, bool kSmall = false>
+MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r, Ctl& k, const Act4& act, int n_act,
                            int32_t* dec, int64_t* met) {
-    int state = r.c[C_STATE];
+    static_assert(!(kGeneral && kSmall), "the small-topology path is noise-free");
+    const bool joint = !kSmall && s.joint;
+    const bool res1 = kSmall || s.res_is_one;
+    int state = k.state;
     int nev = 0;
     if (state >= ST_DONE) {  // StopIteration -> (None, None, True)   core.py:128-131
         g.sync();
+        if (state == ST_DONE) k.state = ST_FINISHED;
         if (g.lane == 0) {
-            if (state == ST_DONE) r.c[C_STATE] = ST_FINISHED;
             int32_t od[8] = {0, 0, 0, 0, 0, 0, 2, 0};
             store_out(dec, met, od, 0, 0, 0);
         }
@@ -1053,33 +1184,35 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
         // _assign_action (core.py:301-315): the decision event finishes, TAKE_ACTION runs as its immediate event
         g.sync();
         int n_apply = n_act;
-        if (s.joint) {  // answer k belongs to the k-th decision of the tick; surplus answers are dropped (zip, core.py:362)
-            const uint64_t pend = ((uint64_t)(uint32_t)r.c[C_ARR_HI] << 32) | (uint32_t)r.c[C_ARR_LO];
+        if (joint) {  // answer k belongs to the k-th decision of the tick; surplus answers are dropped (zip, core.py:362)
+            const uint64_t pend = k.arr;
             int n_dec = 0;
             for (uint64_t m = pend; m; m &= m - 1) n_dec++;
             n_apply = n_act < n_dec ? n_act : n_dec;
         }
-        bool ok = on_actions(s, g, r, act, n_apply);
-        if (g.lane == 0) {
-            ctrl_add64(r, C_NSTEPS_LO, 1);
-            if (!ok) { r.c[C_STATE] = ST_ERROR; r.c[C_ERR] = -1; }
+        const bool ok = g.ballot(!on_actions<G, kSmall>(s, g, r, k, act, n_apply)) == 0;  // (decided by the leader lane)
+        k.nsteps += 1;
+        if (!ok) {
+            k.state = ST_ERROR;
+            if (g.lane == 0) r.c[C_ERR] = -1;
         }
         g.sync();
-        nev += s.joint ? 2 * n_apply : 2;  // decision event + TAKE_ACTION per answered decision
-        if (r.c[C_STATE] == ST_ERROR) {
+        nev += joint ? 2 * n_apply : 2;  // decision event + TAKE_ACTION per answered decision
+        if (!ok) {
             if (g.lane == 0) { int32_t od[8] = {0, 0, 0, 0, 0, 0, -1, 0}; store_out(dec, met, od, 0, 0, 0); }
             g.sync();
             return;
         }
         state = ST_DECISIONS;
     } else {
-        if (g.lane == 0) ctrl_add64(r, C_NSTEPS_LO, 1);
+        k.nsteps += 1;
         if (state == ST_START) state = ST_TICK_BEGIN;
     }
+    PHASE_MARK(r, PH_ACTIONS);
 
-    int tick = r.c[C_TICK];
-    uint64_t arr = ((uint64_t)(uint32_t)r.c[C_ARR_HI] << 32) | (uint32_t)r.c[C_ARR_LO];
-    int dec_pos = r.c[C_DEC_POS];
+    int tick = k.tick;
+    uint64_t arr = k.arr;
+    int dec_pos = k.dec_pos;
     int status = 0, nticks = 0;
     int32_t od[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     for (;;) {
@@ -1093,25 +1226,28 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
             int total_empty = 0;
             int ndep = 0;
             arr = 0;
-            for (int b0 = 0; b0 < s.V; b0 += G) {
+            GROUP_CHUNKS(b0, s.V) {
                 const int v = b0 + g.lane;
                 const bool in = v < s.V;
-                const bool arrives = in && r.c[C_FIXED + 2 * s.V + v] == tick;
+                // the vessel's cursors: dep_cursor (C_FIXED + v), next departure tick (+ V), next arrival tick (+ 2V)
+                int* cur = kSmall ? nullptr : r.c + C_FIXED + v;
+                const bool arrives = in && (kSmall ? k.next_arr : cur[2 * s.V]) == tick;
                 if (arrives) {
                     int si = TBL_I(r, s.t_stop_offset, v) + VA(s, r, VA_NEXT_LOC_IDX, v);
                     r.f[s.o_vp + v * s.P + TBL_I(r, s.t_stop_port, si)] = tick;
-                    r.c[C_FIXED + 2 * s.V + v] = NO_TICK;
+                    if (kSmall) k.next_arr = NO_TICK; else cur[2 * s.V] = NO_TICK;
                 }
                 if (kGeneral && s.order_mode == 1 && in) total_empty += VA(s, r, VA_EMPTY, v);
-                const bool departs = in && r.c[C_FIXED + s.V + v] == tick;
+                const bool departs = in && (kSmall ? k.next_dep : cur[s.V]) == tick;
                 if (departs) {
                     on_departure(s, r, v);
-                    int dc = r.c[C_FIXED + v] + 1;
-                    r.c[C_FIXED + v] = dc;
+                    const int dc = (kSmall ? k.dep_cursor : cur[0]) + 1;
                     int sb = TBL_I(r, s.t_stop_offset, v), ns = TBL_I(r, s.t_stop_offset, v + 1) - sb;
-                    r.c[C_FIXED + s.V + v] = dc < ns ? TBL_I(r, s.t_stop_leave, sb + dc) : NO_TICK;
+                    const int nd = dc < ns ? TBL_I(r, s.t_stop_leave, sb + dc) : NO_TICK;
                     int nl = VA(s, r, VA_NEXT_LOC_IDX, v);
-                    r.c[C_FIXED + 2 * s.V + v] = nl < ns ? TBL_I(r, s.t_stop_arrival, sb + nl) : NO_TICK;
+                    const int na = nl < ns ? TBL_I(r, s.t_stop_arrival, sb + nl) : NO_TICK;
+                    if (kSmall) { k.dep_cursor = dc; k.next_dep = nd; k.next_arr = na; }
+                    else { cur[0] = dc; cur[s.V] = nd; cur[2 * s.V] = na; }
                 }
                 arr |= (uint64_t)g.ballot(arrives) << b0;
                 ndep += maro_popc(g.ballot(departs));
@@ -1122,32 +1258,37 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
             }
             nev += ndep;
             g.sync();
+            PHASE_MARK(r, PH_VESSELS);
             // ---- (b) events queued by earlier ticks
-            nev += run_bucket<G, kGeneral>(s, g, r, tick);
-            if (!kGeneral && s.DL) nev += run_delay_line(s, g, r, tick);
+            nev += run_bucket<G, kGeneral, kSmall>(s, g, r, tick);
+            PHASE_MARK(r, PH_BUCKET);
+            if (!kGeneral && (kSmall || s.DL)) nev += run_delay_line<G, kSmall>(s, g, r, tick);
+            PHASE_MARK(r, PH_DELAY);
             // ---- (c) this tick's orders
             if (!kGeneral || s.order_table) {
                 int slot = TBL_I(r, s.t_ord_slot, tick);
                 int lo = TBL_I(r, s.t_ord_off, slot), hi = TBL_I(r, s.t_ord_off, slot + 1);
                 const int32_t* list = r.t + s.t_ord_list + 2 * lo;
-                nev += run_orders<G, kGeneral>(s, g, r, tick, hi - lo, [&](int i, int& w, int& q) { w = list[2 * i]; q = list[2 * i + 1]; });
+                nev += run_orders<G, kGeneral, kSmall>(s, g, r, tick, hi - lo, [&](int i, int& w, int& q) { w = list[2 * i]; q = list[2 * i + 1]; });
             } else {
                 // float64 generation on the leader lane into the replica's scratch area, then cooperative execution
                 int32_t* olist = reinterpret_cast<int32_t*>(r.mt + s.mt_scratch + 64);
                 double* dscr = reinterpret_cast<double*>(olist + 2 * ((s.max_targets + 1) & ~1));
                 g.sync();
                 int n = gen_orders_coop(s, g, r, tick, total_empty, olist, dscr);
-                nev += run_orders<G, kGeneral>(s, g, r, tick, n, [&](int i, int& w, int& q) { w = olist[2 * i]; q = olist[2 * i + 1]; });
+                nev += run_orders<G, kGeneral, kSmall>(s, g, r, tick, n, [&](int i, int& w, int& q) { w = olist[2 * i]; q = olist[2 * i + 1]; });
             }
             g.sync();
+            PHASE_MARK(r, PH_ORDERS);
             // ---- (d) VESSEL_ARRIVAL + LOAD_FULL per arriving vessel, vessel order
             uint64_t m = arr;
             while (m) {
                 int v = maro_ffs64(m) - 1;
                 m &= m - 1;
-                run_arrival(s, g, r, tick, v);
+                run_arrival<G, kSmall>(s, g, r, tick, v);
                 nev += 2;
             }
+            PHASE_MARK(r, PH_ARRIVALS);
             dec_pos = 0;
             state = ST_DECISIONS;
         }
@@ -1155,7 +1296,7 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
         uint64_t m = dec_pos >= 64 ? 0 : (arr >> dec_pos) << dec_pos;
         if (m) {
             int v = maro_ffs64(m) - 1;
-            take_snapshot(s, g, r, frame_index_of(s, tick));  // core.py:345
+            take_snapshot(s, g, r, k, frame_index_of<kSmall>(s, tick));  // core.py:345
             if (g.lane == 0) {
                 int port = VA(s, r, VA_LOC_PORT_IDX, v);
                 int pe = PA(s, r, PA_EMPTY, port), sp = VA(s, r, VA_REMAINING_SPACE, v);
@@ -1163,28 +1304,29 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
                 od[3] = pe < sp ? pe : sp;
                 od[4] = VA(s, r, VA_EMPTY, v);
                 od[5] = VA(s, r, VA_EARLY_DISCHARGE, v);
-                if (s.joint) {  // rows 1.. : the tick's other decisions, scopes from the same (pre-action) state; then a terminator
-                    int k = 1;
-                    for (uint64_t rest = m & (m - 1); rest; rest &= rest - 1, k++) {
+                if (joint) {  // rows 1.. : the tick's other decisions, scopes from the same (pre-action) state; then a terminator
+                    int n = 1;
+                    for (uint64_t rest = m & (m - 1); rest; rest &= rest - 1, n++) {
                         const int v2 = maro_ffs64(rest) - 1, port2 = VA(s, r, VA_LOC_PORT_IDX, v2);
                         const int pe2 = PA(s, r, PA_EMPTY, port2), sp2 = VA(s, r, VA_REMAINING_SPACE, v2);
                         int32_t row[8] = {tick, port2, v2, pe2 < sp2 ? pe2 : sp2, VA(s, r, VA_EMPTY, v2), VA(s, r, VA_EARLY_DISCHARGE, v2),
-                                          0, r.c[C_EP_STEP]};
-                        for (int i = 0; i < 8; i++) dec[8 * k + i] = row[i];
+                                          0, k.ep_step};
+                        for (int i = 0; i < 8; i++) dec[8 * n + i] = row[i];
                     }
-                    if (k < s.V) dec[8 * k + 6] = 3;  // MARO_STATUS_INACTIVE: end of this step's decision list
+                    if (n < s.V) dec[8 * n + 6] = 3;  // MARO_STATUS_INACTIVE: end of this step's decision list
                 }
             }
-            dec_pos = s.joint ? 64 : v + 1;
+            dec_pos = joint ? 64 : v + 1;
             state = ST_AWAIT;
             status = 0;
+            PHASE_MARK(r, PH_DECISION);
             break;
         }
         // ---- post_step (business_engine.py:201-224)
-        if (s.res_is_one || (tick + 1) % s.resolution == 0) {
+        if (res1 || (tick + 1) % s.resolution == 0) {
             g.sync();
             LANE_DIM(p, s.P) PA(s, r, PA_ACC_FULFILLMENT, p) = PA(s, r, PA_ACC_BOOKING, p) - PA(s, r, PA_ACC_SHORTAGE, p);
-            take_snapshot(s, g, r, frame_index_of(s, tick));
+            take_snapshot(s, g, r, k, frame_index_of<kSmall>(s, tick));
             snapshot_wait(g);  // the row has left the frame: the per-tick resets may overwrite it
             LANE_DIM(p, s.P) {
                 PA(s, r, PA_SHORTAGE, p) = 0;
@@ -1195,14 +1337,16 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
             g.sync();
         }
         if (tick + 1 == s.max_tick) {
-            if (!s.res_is_one && (tick + 1) % s.resolution != 0) { take_snapshot(s, g, r, frame_index_of(s, tick)); snapshot_wait(g); }  // core.py:376-378
+            if (!res1 && (tick + 1) % s.resolution != 0) { take_snapshot(s, g, r, k, frame_index_of(s, tick)); snapshot_wait(g); }  // core.py:376-378
             state = ST_DONE;
             status = 1;
             od[0] = tick;
+            PHASE_MARK(r, PH_POST);
             break;
         }
         tick += 1;
         state = ST_TICK_BEGIN;
+        PHASE_MARK(r, PH_POST);
     }
     // ---- metrics (business_engine.py:270-282) + control write-back
     g.sync();
@@ -1215,22 +1359,31 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
         bk = g.sum64(bk);
         sh = g.sum64(sh);
     }
-    if (g.lane == 0) {
-        int err = r.c[C_ERR];
-        if (err == -2) { state = ST_ERROR; status = -2; }
-        r.c[C_STATE] = state;
-        r.c[C_TICK] = tick;
-        r.c[C_ARR_LO] = (int32_t)(uint32_t)(arr & 0xffffffffu);
-        r.c[C_ARR_HI] = (int32_t)(uint32_t)(arr >> 32);
-        r.c[C_DEC_POS] = dec_pos;
-        ctrl_add64(r, C_NEVENTS_LO, nev);
-        ctrl_add64(r, C_NTICKS_LO, nticks);
-        od[6] = status;
-        od[7] = r.c[C_EP_STEP];  // ordinal of this env-step inside the episode (0 = first decision)
-        r.c[C_EP_STEP] += 1;
-        store_out(dec, met, od, bk, sh, ctrl_get64(r, C_OPNUM_LO));
-    }
+    if (r.c[C_ERR] == -2) { state = ST_ERROR; status = -2; }
+    k.state = state;
+    k.tick = tick;
+    k.arr = arr;
+    k.dec_pos = dec_pos;
+    k.nevents += nev;
+    k.nticks += nticks;
+    od[6] = status;
+    od[7] = k.ep_step;  // ordinal of this env-step inside the episode (0 = first decision)
+    k.ep_step += 1;
+    if (g.lane == 0) store_out(dec, met, od, bk, sh, k.opnum);
     snapshot_wait(g);  // the pre-decision snapshot (if any) has been read: the caller may touch the frame again
+    PHASE_COUNT(r, PH_TICKS, nticks);
+    PHASE_MARK(r, PH_STORE);
+}
+
+// One step on the control block as it stands in memory (ctl_load, replica_step, ctl_store): the form for callers that do
+// not keep the control state in registers between steps.
+template <int G, bool kGeneral>
+MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r, const Act4& act, int n_act, int32_t* dec,
+                           int64_t* met) {
+    Ctl k;
+    ctl_load<G, false>(s, g, r, k);
+    replica_step<G, kGeneral, false>(s, g, r, k, act, n_act, dec, met);
+    ctl_store<G, false>(s, g, r, k);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -46,8 +46,15 @@ __device__ __forceinline__ Replica make_replica(const CimShape& s, const StepArg
     r.mt = a.mt ? a.mt + (int64_t)rep * a.mt_words : nullptr;
     r.snap = a.snap + (int64_t)rep * s.ring_rows * s.FWp;
     r.snap_frame = a.snap_frame + (int64_t)rep * s.ring_rows;
+#ifdef MARO_PHASE_CLOCKS
+    r.pc = nullptr;
+#endif
     return r;
 }
+
+#ifdef MARO_PHASE_CLOCKS
+__device__ unsigned long long maro_phase_clk[PH_SLOTS];  // summed over the replicas of every resident rollout
+#endif
 
 // kSpread (small batches, G < 32): one replica per WARP, only its first G lanes work.  Packing 32/G replicas into a warp
 // makes the warp issue the union of their control paths; with fewer replicas than the GPU has warp slots it is faster to
@@ -198,7 +205,8 @@ __device__ __forceinline__ uint4 ld_sys_v4(const uint32_t* p) {
 #ifndef MARO_RES_DENSE_BLOCKS
 #define MARO_RES_DENSE_BLOCKS 3
 #endif
-template <int G, bool kGeneral, int kMinBlocks = 1>
+// kSmall: the small-topology instantiation of replica_step (cim_small_ok), chosen per handle at create (res_small).
+template <int G, bool kGeneral, int kMinBlocks = 1, bool kSmall = false>
 __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __grid_constant__ CimShape s, const __grid_constant__ StepArgs a,
                                                            const __grid_constant__ ResidentArgs ra) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -260,6 +268,8 @@ __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __g
     while (!mbar_try_wait(bar, phase)) {}
     phase ^= 1u;
     Replica r = make_replica(s, a, rep, st);
+    Ctl k;  // the control state stays in registers until the write-back below
+    ctl_load<G, kSmall>(s, g, r, k);
     int32_t* gdec = a.decisions + (int64_t)rep * 8;
     int64_t* gmet = a.metrics + (int64_t)rep * 3;
 
@@ -267,10 +277,17 @@ __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __g
         if (g.lane < 8) dslot[g.lane] = gdec[g.lane];  // the decision the previous launch / slice returned (feeds the agent)
         if (slice > 0 && g.lane < 3) mslot[g.lane] = gmet[g.lane];
         g.sync();
-        int k = k_begin;
+        int step = k_begin;
         // (a later slice of a replica whose episode ended in an earlier one: nothing left to do but the trace rows)
         const bool over = slice > 0 && (dslot[MARO_DEC_STATUS] == MARO_STATUS_FINISHED || dslot[MARO_DEC_STATUS] == MARO_STATUS_DONE);
-        for (; k < k_end && !over; k++) {
+#ifdef MARO_PHASE_CLOCKS
+        PhaseClk pclk;
+        for (int i = 0; i < PH_SLOTS; i++) pclk.acc[i] = 0;
+        pclk.t = clock64();
+        r.pc = &pclk;
+#endif
+        for (; step < k_end && !over; step++) {
+            PHASE_MARK(r, PH_STORE);  // (the previous step's trace row and status test)
             Act4 act = {0, 0, 0, 0};
             int n_act = 0;
             if (ra.policy == RES_POLICY_RANDOM) {
@@ -280,18 +297,26 @@ __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __g
                     act.v = o.x; act.p = o.y; act.qty = o.z; act.type = o.w;
                 }
             }
-            replica_step<G, kGeneral>(s, g, r, act, n_act, dslot, mslot);
+            PHASE_MARK(r, PH_AGENT);
+            PHASE_COUNT(r, PH_STEPS, 1);
+            replica_step<G, kGeneral, kSmall>(s, g, r, k, act, n_act, dslot, mslot);
             if (ra.trace && g.lane < 2)
-                reinterpret_cast<int4*>(ra.trace + ((int64_t)k * s.n_replicas + rep) * 8)[g.lane] = reinterpret_cast<const int4*>(dslot)[g.lane];
+                reinterpret_cast<int4*>(ra.trace + ((int64_t)step * s.n_replicas + rep) * 8)[g.lane] = reinterpret_cast<const int4*>(dslot)[g.lane];
             const int status = dslot[MARO_DEC_STATUS];
             // the episode is over: stop here and keep the DONE row with the final metrics (a further step — in this launch
             // or the next — returns the all-zero FINISHED row, core.py:128-131)
-            if (status == MARO_STATUS_FINISHED || status == MARO_STATUS_DONE) { k++; break; }
+            if (status == MARO_STATUS_FINISHED || status == MARO_STATUS_DONE) { step++; break; }
         }
+#ifdef MARO_PHASE_CLOCKS
+        PHASE_MARK(r, PH_STORE);
+        if (g.lane == 0)
+            for (int i = 0; i < PH_SLOTS; i++) atomicAdd(&maro_phase_clk[i], pclk.acc[i]);
+        r.pc = nullptr;
+#endif
         if (ra.trace)
-            for (; k < k_end; k++)
+            for (; step < k_end; step++)
                 if (g.lane < 2)
-                    reinterpret_cast<int4*>(ra.trace + ((int64_t)k * s.n_replicas + rep) * 8)[g.lane] = reinterpret_cast<const int4*>(dslot)[g.lane];
+                    reinterpret_cast<int4*>(ra.trace + ((int64_t)step * s.n_replicas + rep) * 8)[g.lane] = reinterpret_cast<const int4*>(dslot)[g.lane];
         if (g.lane < 2) reinterpret_cast<int4*>(gdec)[g.lane] = reinterpret_cast<const int4*>(dslot)[g.lane];
         if (g.lane < 3) gmet[g.lane] = mslot[g.lane];
     } else {
@@ -362,8 +387,9 @@ __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __g
             const int n_act = min((int)(flags & 0xff), min(s.max_actions, G));
             const bool active = (flags >> 8) & 1u, bad = (flags >> 9) & 1u;
             if ((flags >> 10) & 1u) {  // Env.reset of this replica (maro_cim_reset while the session is live), in place
+                ctl_store<G, kSmall>(s, g, r, k);  // (the work counters in registers survive the reset)
                 replica_reset<G>(s, g, r);
-                g.sync();
+                ctl_load<G, kSmall>(s, g, r, k);
             }
             if (active) {
                 Act4 act = {0, 0, 0, 0};
@@ -374,7 +400,7 @@ __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __g
                     uint4 v = ld_sys_v4(reinterpret_cast<const uint32_t*>(a.actions + ((int64_t)rep * s.max_actions + g.lane) * 4));
                     act.v = (int)v.x; act.p = (int)v.y; act.qty = (int)v.z; act.type = (int)v.w;
                 }
-                replica_step<G, kGeneral>(s, g, r, act, n_act, dslot, mslot);
+                replica_step<G, kGeneral, kSmall>(s, g, r, k, act, n_act, dslot, mslot);
             } else if (g.lane == 0) {
                 dslot[MARO_DEC_STATUS] = MARO_STATUS_INACTIVE;
             }
@@ -390,8 +416,8 @@ __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __g
                 uint32_t w[3];
 #pragma unroll
                 for (int i = 0; i < 3; i++) {
-                    const int k = 3 * g.lane + i;
-                    w[i] = k < 14 ? p[k] : 0u;
+                    const int wi = 3 * g.lane + i;
+                    w[i] = wi < 14 ? p[wi] : 0u;
                 }
                 asm volatile("st.relaxed.sys.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(ra.results + (int64_t)rep * MARO_RES_LINE_WORDS + g.lane * 4),
                              "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(expect)
@@ -403,6 +429,7 @@ __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __g
         for (int i = g.lane; i < 16; i += G) ra.rows[(int64_t)rep * 16 + i] = dslot[i];
     }
     // ---- write back the block + the light-step hint of the per-step kernel
+    ctl_store<G, kSmall>(s, g, r, k);
     if (g.lane == 0) snapshot_drain_lane();
     g.sync();
     const int4* src4 = reinterpret_cast<const int4*>(st);
@@ -438,6 +465,7 @@ struct MaroCimEnv : EnvCommon {
     std::vector<int32_t> h_tables;
     // resident mode (cim_resident_kernel)
     int res_threads = 0, res_grid = 0, res_spread = 0, res_dense = 0;
+    int res_small = 0;                               // the resident kernel runs the small-topology instantiation (cim_small_ok)
     size_t res_smem = 0;
     bool session_ok = false;                         // the whole grid is co-resident (required to spin-wait)
     std::atomic<bool> session_live{false};
@@ -653,6 +681,7 @@ static cudaError_t launch_resident_g(MaroCimEnv* e, const StepArgs& a, const Res
         return cudaGetLastError();
     };
     if (general) return go(cim_resident_kernel<G, true>);
+    if (e->res_small) return go(cim_resident_kernel<G, false, 1, true>);
     return e->res_dense ? go(cim_resident_kernel<G, false, MARO_RES_DENSE_BLOCKS>) : go(cim_resident_kernel<G, false>);
 }
 
@@ -896,7 +925,18 @@ static int create_device_side(MaroCimEnv* e, const MaroCimTopology* topos, int32
         StepArgs a = base_args(e);
         ResidentArgs ra;
         memset(&ra, 0, sizeof(ra));
+        e->res_small = 0;
         CK(launch_resident(e, a, ra, session_geom(e), true, &per_sm));
+        // the small-topology instantiation where the shape allows it (MARO_B200_RES_SMALL=0/1 forces it off / on where allowed),
+        // never in place of the register-capped one and never where it would hold fewer CTAs per SM
+        const char* rsm = getenv("MARO_B200_RES_SMALL");
+        if (cim_small_ok(s, e->lanes) && (rsm ? atoi(rsm) != 0 : !e->res_dense)) {
+            int per_sm_small = 0;
+            e->res_small = 1;
+            CK(launch_resident(e, a, ra, session_geom(e), true, &per_sm_small));
+            if (per_sm_small < per_sm && !rsm) e->res_small = 0;
+            else per_sm = per_sm_small;
+        }
         e->res_per_sm = per_sm;
         if (attempt == 0 && e->res_spread && !rs && gpw > 1 && (int64_t)per_sm * nsm < e->res_grid) {
             e->res_spread = 0;
@@ -1261,6 +1301,20 @@ int maro_cim_rollout_device(MaroCimEnv* e, int32_t policy, uint32_t seed, uint32
     CK(launch_resident(e, a, ra, geo));
     return 0;
 }
+
+#ifdef MARO_PHASE_CLOCKS
+// (-DMARO_PHASE_CLOCKS builds only, tools/phase_clocks.py) copy the phase accumulators of the device to `out` [PH_SLOTS],
+// then zero them if `clear`.  Synchronises the device.
+int maro_cim_phase_clocks(uint64_t* out, int32_t clear) {
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpyFromSymbol(out, maro_phase_clk, sizeof(unsigned long long) * PH_SLOTS));
+    if (clear) {
+        static const unsigned long long zero[PH_SLOTS] = {};
+        CK(cudaMemcpyToSymbol(maro_phase_clk, zero, sizeof(zero)));
+    }
+    return 0;
+}
+#endif
 
 int maro_cim_random_policy_device(MaroCimEnv* e, const int32_t* d_decisions, int32_t* d_actions, uint32_t seed,
                                   uint32_t replica_base) {

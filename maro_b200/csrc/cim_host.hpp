@@ -323,4 +323,12 @@ inline int lanes_per_replica(const CimShape& s) {
     return w <= 8 ? 8 : (w <= 16 ? 16 : 32);
 }
 
+// May replica_step<G, false, kSmall = true> run this shape with G lanes per replica?  Noise-free fixed-order mode with
+// integer buffer ticks (the kGeneral = false path), snapshot resolution 1, container volume 1, Sequential mode, delay
+// lines on, and every dimension a lane loop runs over (ports, vessels, route stops, future stops) <= G.
+inline bool cim_small_ok(const CimShape& s, int G) {
+    return s.order_table && !s.order_noise && !s.buffer_noise && s.res_is_one && s.vol_is_one && !s.joint && s.DL > 0 &&
+           s.P <= G && s.V <= G && s.max_route_len <= G && s.fut <= G;
+}
+
 }  // namespace maro
