@@ -201,7 +201,7 @@ enum Ctrl {
     C_OPNUM_LO, C_OPNUM_HI, C_MT_ORDER_IDX, C_MT_BUFFER_IDX,
     C_NSTEPS_LO, C_NSTEPS_HI, C_NTICKS_LO, C_NTICKS_HI, C_NEVENTS_LO, C_NEVENTS_HI, C_NSNAPS_LO, C_NSNAPS_HI,
     C_LAST_FRAME, C_N_ORDERS, C_EP_STEP, C_RESERVED2,
-    C_FIXED  // followed by dep_cursor[V], next_dep_tick[V], next_arr_tick[V]
+    C_FIXED  // followed by dep_cursor[V], next_dep_tick[V], next_arr_tick[V] (+ due_stop[V], due_tick[V] with due rings)
 };
 #define NO_TICK 0x7fffffff
 enum State { ST_START = 0, ST_TICK_BEGIN = 1, ST_DECISIONS = 2, ST_AWAIT = 3, ST_DONE = 4, ST_FINISHED = 5, ST_ERROR = 6 };
@@ -234,6 +234,12 @@ struct CimShape {
     // slot (tick & (DL-1)) = { rf[P*P] (src*P+dst -> quantity), re[P] (port -> quantity), n_rf, n_re (event counts) } at word
     // offset o_dl of the state block.  Same arithmetic, same event counts, no list walking / free list / push machinery.
     int DL, o_dl, dl_stride;
+    // Due rings (delay-line handles whose every vessel visits its stops at strictly increasing ticks; 0 = off, the calendar
+    // queue carries DISCHARGE_FULL): the discharges LOAD_FULL schedules are pure adds due at a known stop of the loading vessel,
+    // so they are ACCUMULATED per (vessel, stop) instead of queued: vessel v's ring of due_R slots {quantity, events} at word
+    // offset o_due + 2 * due_R * v, slot = stop index & (due_R - 1), due_R = power of two > max_route_len.  The control
+    // block holds each vessel's next due stop and its arrival tick (C_FIXED + 3V + v, + 4V + v; kSmall: Ctl on lane v).
+    int due_R, o_due;
     // DecisionMode.Joint (core.py:354-366): every decision event of a tick is returned at once (V rows of 8 words), the
     // answers are applied in list order when the replica is stepped again.  DW = words of a replica's decision block.
     int joint, DW;
@@ -293,18 +299,23 @@ MARO_DEV void ctrl_add64(const Replica& r, int lo, int64_t d) { ctrl_set64(r, lo
 // Control state that replica_step reads or writes on every step, held in registers for as long as the block stays on the SM
 // (a resident launch: loaded once after stage-in, stored once before write-back; other callers around each call).  The
 // scalars are the same in every lane of the group; the 64-bit counters are kept by the leader lane.  In the small-topology
-// instantiation (kSmall: V <= G) lane v also holds vessel v's three cursors C_FIXED + {0, V, 2V} + v.  What stays in the
-// control block (free stack top, error word, MT19937 positions, ...) is shared-memory state of the phases that use it.
+// instantiation (kSmall: V <= G) lane v also holds vessel v's five cursors C_FIXED + {0, V, 2V, 3V, 4V} + v.  What stays in
+// the control block (free stack top, error word, MT19937 positions, ...) is shared-memory state of the phases that use it.
 // ------------------------------------------------------------------------------------------------
 struct Ctl {
     int state, tick, dec_pos, ep_step, last_frame;
     uint64_t arr;  // vessels arriving this tick (C_ARR_LO / C_ARR_HI)
     int64_t opnum, nsteps, nticks, nevents, nsnaps;
+    int64_t ndue;  // events the due rings executed on THIS lane (per-lane partial count, added to C_NEVENTS by ctl_store)
     int dep_cursor, next_dep, next_arr;  // kSmall: vessel g.lane's cursors (NO_TICK on lanes >= V)
+    int due_stop, due_tick;              // kSmall: vessel g.lane's next due stop and its arrival tick (NO_TICK on lanes >= V)
+    bool snap_pending;  // deferred pre-decision snapshot not written yet (fused rollouts, replica_step<..., kDeferSnap>)
 };
 
 template <int G, bool kSmall>
 MARO_DEV void ctl_load(const CimShape& s, const Grp<G>& g, const Replica& r, Ctl& k) {
+    k.ndue = 0;
+    k.snap_pending = false;
     k.state = r.c[C_STATE];
     k.tick = r.c[C_TICK];
     k.dec_pos = r.c[C_DEC_POS];
@@ -321,11 +332,16 @@ MARO_DEV void ctl_load(const CimShape& s, const Grp<G>& g, const Replica& r, Ctl
     k.dep_cursor = in ? r.c[C_FIXED + v] : 0;
     k.next_dep = in ? r.c[C_FIXED + s.V + v] : NO_TICK;
     k.next_arr = in ? r.c[C_FIXED + 2 * s.V + v] : NO_TICK;
+    k.due_stop = in ? r.c[C_FIXED + 3 * s.V + v] : 0;
+    k.due_tick = in ? r.c[C_FIXED + 4 * s.V + v] : NO_TICK;
 }
 
 // (ends with a group barrier: the control block is complete for every lane afterwards)
 template <int G, bool kSmall>
-MARO_DEV void ctl_store(const CimShape& s, const Grp<G>& g, const Replica& r, const Ctl& k) {
+MARO_DEV void ctl_store(const CimShape& s, const Grp<G>& g, const Replica& r, Ctl& k) {
+    const int64_t ndue = g.sum64(k.ndue);
+    k.nevents += ndue;  // (every lane: the partials restart from zero)
+    k.ndue = 0;
     g.sync();
     if (g.lane == 0) {
         r.c[C_STATE] = k.state;
@@ -346,6 +362,8 @@ MARO_DEV void ctl_store(const CimShape& s, const Grp<G>& g, const Replica& r, co
         r.c[C_FIXED + v] = k.dep_cursor;
         r.c[C_FIXED + s.V + v] = k.next_dep;
         r.c[C_FIXED + 2 * s.V + v] = k.next_arr;
+        r.c[C_FIXED + 3 * s.V + v] = k.due_stop;
+        r.c[C_FIXED + 4 * s.V + v] = k.due_tick;
     }
     g.sync();
 }
@@ -456,6 +474,43 @@ MARO_DEV uint16_t* q_next(const CimShape& s, const Replica& r) { return reinterp
 MARO_DEV uint16_t* q_free(const CimShape& s, const Replica& r) { return q_next(s, r) + s.QN; }
 
 MARO_DEV int32_t* dl_slot(const CimShape& s, const Replica& r, int tick) { return r.f + s.o_dl + (tick & (s.DL - 1)) * s.dl_stride; }
+
+// Due-ring slot {quantity, events} of vessel v's stop `stop`.  No two outstanding stops of a vessel share a slot: LOAD_FULL at
+// stop `loc` schedules discharges at stops loc + 1 .. loc + rl only (rl = the vessel's route length), and the drain cursor has
+// passed every stop up to the vessel's latest arrival (stop ticks increase strictly, the drain of tick T runs before that
+// tick's arrivals).  So the outstanding stops of a vessel lie in (loc, loc + rl] for its latest arrival stop loc -- at most
+// rl < due_R consecutive stop indices.
+MARO_DEV int32_t* due_slot(const CimShape& s, const Replica& r, int v, int stop) {
+    return r.f + s.o_due + 2 * (v * s.due_R + (stop & (s.due_R - 1)));
+}
+
+// Phase (b) for the due rings, vessel v (one lane): the DISCHARGE_FULL events (:658-693) accumulated for its stop `stop`,
+// due at `tick`, and the RETURN_EMPTY each of them creates -- the arithmetic of run_bucket's discharge branch on the summed
+// quantity.  Immediate returns (empty-return buffer 0) cancel on on_consignee.  Returns the events executed.
+MARO_DEV int drain_due_stop(const CimShape& s, const Replica& r, int v, int stop, int tick) {
+    int32_t* sl = due_slot(s, r, v, stop);
+    const int n = sl[1];
+    if (n == 0) return 0;
+    const int qty = sl[0];
+    sl[0] = 0;
+    sl[1] = 0;
+    const int port = TBL_I(r, s.t_stop_port, TBL_I(r, s.t_stop_offset, v) + stop);
+    VA(s, r, VA_FULL, v) -= qty;
+    VA(s, r, VA_REMAINING_SPACE, v) += qty;
+    r.f[s.o_fov + v * s.P + port] -= qty;
+    const int buf = TBL_I(r, s.t_erb_i, port);
+    if (buf == 0) {
+        atomic_add(&PA(s, r, PA_EMPTY, port), qty);
+        return 2 * n;
+    }
+    atomic_add(&PA(s, r, PA_ON_CONSIGNEE, port), qty);
+    if (tick + buf < s.max_tick) {
+        int32_t* dl = dl_slot(s, r, tick + buf);
+        atomic_add(&dl[s.P * s.P + port], qty);
+        atomic_add(&dl[s.P * s.P + s.P + 1], n);
+    }
+    return n;
+}
 
 // Drain the delay-line slot of `tick`: every accumulated RETURN_FULL (:499-522) and RETURN_EMPTY (:695-706) of this tick.
 // kSmall (P <= G): lane p drains source port p's row and port p's RETURN_EMPTY entry, then applies the row's total to port p
@@ -961,7 +1016,7 @@ MARO_DEV int gen_orders_coop(const CimShape& s, const Grp<G>& g, const Replica& 
 // ------------------------------------------------------------------------------------------------
 // Phase (d): VESSEL_ARRIVAL (:600-632) + LOAD_FULL (:524-598) of one arriving vessel, lanes over route positions.
 // ------------------------------------------------------------------------------------------------
-template <int G, bool kSmall>
+template <int G, bool kGeneral, bool kSmall>
 MARO_DEV void run_arrival(const CimShape& s, const Grp<G>& g, const Replica& r, int tick, int v) {
     const int loc = VA(s, r, VA_NEXT_LOC_IDX, v);
     const int sb = TBL_I(r, s.t_stop_offset, v);
@@ -1018,8 +1073,17 @@ MARO_DEV void run_arrival(const CimShape& s, const Grp<G>& g, const Replica& r, 
             r.f[s.o_fop + port * s.P + next_port] = pending - loaded;
             r.f[s.o_fov + v * s.P + next_port] += loaded;
         }
-        group_push(s, g, r, loaded > 0, tick, valid ? TBL_I(r, s.t_stop_arrival, sb + si) : 0,
-                   DE_DISCHARGE_FULL | (v << 8) | (port << 16) | (next_port << 24), loaded);
+        if (!kGeneral && (kSmall || s.due_R)) {  // lanes hold distinct stops: plain adds; the drop rules of group_push
+            if (loaded > 0 && TBL_I(r, s.t_stop_arrival, sb + si) < s.max_tick) {
+                int32_t* sl = due_slot(s, r, v, si);
+                sl[0] += loaded;
+                sl[1] += 1;
+            }
+            if (!kSmall) g.sync();  // (a later chunk may read the pending cargo this one wrote)
+        } else {
+            group_push(s, g, r, loaded > 0, tick, valid ? TBL_I(r, s.t_stop_arrival, sb + si) : 0,
+                       DE_DISCHARGE_FULL | (v << 8) | (port << 16) | (next_port << 24), loaded);
+        }
         int chunk = g.shfl(hi, G - 1);
         total_loaded += chunk;
         acceptable -= chunk;
@@ -1058,6 +1122,11 @@ MARO_DEV void on_departure(const CimShape& s, const Replica& r, int v) {
 }
 
 struct Act4 { int32_t v, p, qty, type; };
+
+template <bool kSmall = false>
+MARO_DEV int frame_index_of(const CimShape& s, int tick) {
+    return kSmall || s.res_is_one ? tick - s.start_tick : (tick - s.start_tick) / s.resolution;
+}
 
 // _on_action_received (:708-748).  Lane k holds action k (loaded with one 128-bit read); the leader lane applies them in
 // order.  Returns false where the reference would raise AssertionError.
@@ -1111,8 +1180,9 @@ MARO_DEV void snapshot_wait(const Grp<G>& g) {
     g.sync();
 }
 
+// the copy of the frame into its ring row (take_snapshot without the counters)
 template <int G>
-MARO_DEV void take_snapshot(const CimShape& s, const Grp<G>& g, const Replica& r, Ctl& k, int frame_index) {
+MARO_DEV void snapshot_store(const CimShape& s, const Grp<G>& g, const Replica& r, int frame_index) {
     int row = frame_index < s.ring_rows ? frame_index : frame_index % s.ring_rows;
     int32_t* dst = r.snap + (int64_t)row * s.FWp;
 #ifdef MARO_HOST_EMULATION
@@ -1133,8 +1203,26 @@ MARO_DEV void take_snapshot(const CimShape& s, const Grp<G>& g, const Replica& r
     }
 #endif
     if (g.lane == 0) r.snap_frame[row] = frame_index;
+}
+
+template <int G>
+MARO_DEV void take_snapshot(const CimShape& s, const Grp<G>& g, const Replica& r, Ctl& k, int frame_index) {
+    snapshot_store(s, g, r, frame_index);
     k.last_frame = frame_index;
     k.nsnaps += 1;
+    k.snap_pending = false;  // (a pending pre-decision snapshot is always of this frame index: same row, now overwritten)
+}
+
+// Fused rollouts (replica_step<..., kDeferSnap = true>) take the pre-decision snapshot only logically: inside a launch its ring
+// row is always overwritten before anything can read it -- the decision's tick ends with the snapshot of the same frame index
+// (same row), and between the two only the device agent runs, which reads the decision row, never the ring.  The row becomes
+// observable only if the launch (or slice) ends while the replica waits on that decision; then the frame is still exactly the
+// pre-decision frame (nothing modifies it after the decision), and this writes it.  Call once per work item before the write-back.
+template <int G, bool kSmall>
+MARO_DEV void flush_deferred_snapshot(const CimShape& s, const Grp<G>& g, const Replica& r, Ctl& k) {
+    if (!k.snap_pending) return;  // (group-uniform)
+    snapshot_store(s, g, r, frame_index_of<kSmall>(s, k.tick));
+    k.snap_pending = false;
 }
 
 // Output rows are written with 128-bit / 64-bit stores (they may live in mapped host memory: one PCIe write each).
@@ -1148,11 +1236,6 @@ MARO_DEV void store_out(int32_t* dec, int64_t* met, const int32_t* od, int64_t m
     met[0] = m0; met[1] = m1; met[2] = m2;
 }
 
-template <bool kSmall = false>
-MARO_DEV int frame_index_of(const CimShape& s, int tick) {
-    return kSmall || s.res_is_one ? tick - s.start_tick : (tick - s.start_tick) / s.resolution;
-}
-
 // ------------------------------------------------------------------------------------------------
 // One Env.step for one replica.  `act`/`n_act` are this replica's action rows; `dec` (8 int32) and `met`
 // (3 int64) its output rows.  All lanes of the group call this together.
@@ -1162,12 +1245,14 @@ MARO_DEV int frame_index_of(const CimShape& s, int tick) {
 // lines on, and P, V, route lengths and fut <= G (cim_small_ok) -- every lane loop over them is one pass, the vessel cursors
 // live in Ctl.  Sizes and table offsets stay runtime values.
 // The control state is `k` (ctl_load before, ctl_store after: the control block in shared memory is stale in between).
-template <int G, bool kGeneral, bool kSmall = false>
+// kDeferSnap (fused rollouts only): the pre-decision snapshot is left pending in `k` (flush_deferred_snapshot).
+template <int G, bool kGeneral, bool kSmall = false, bool kDeferSnap = false>
 MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r, Ctl& k, const Act4& act, int n_act,
                            int32_t* dec, int64_t* met) {
     static_assert(!(kGeneral && kSmall), "the small-topology path is noise-free");
     const bool joint = !kSmall && s.joint;
     const bool res1 = kSmall || s.res_is_one;
+    const bool due = !kGeneral && (kSmall || s.due_R);  // discharges on the due rings instead of the calendar queue
     int state = k.state;
     int nev = 0;
     if (state >= ST_DONE) {  // StopIteration -> (None, None, True)   core.py:128-131
@@ -1249,6 +1334,15 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
                     if (kSmall) { k.dep_cursor = dc; k.next_dep = nd; k.next_arr = na; }
                     else { cur[0] = dc; cur[s.V] = nd; cur[2 * s.V] = na; }
                 }
+                // (b) for the due rings: the discharges due at this stop (fields disjoint from the departure's)
+                if (due && in && (kSmall ? k.due_tick : cur[4 * s.V]) == tick) {
+                    const int stop = kSmall ? k.due_stop : cur[3 * s.V];
+                    k.ndue += drain_due_stop(s, r, v, stop, tick);
+                    const int sb = TBL_I(r, s.t_stop_offset, v), ns = TBL_I(r, s.t_stop_offset, v + 1) - sb;
+                    const int nt = stop + 1 < ns ? TBL_I(r, s.t_stop_arrival, sb + stop + 1) : NO_TICK;
+                    if (kSmall) { k.due_stop = stop + 1; k.due_tick = nt; }
+                    else { cur[3 * s.V] = stop + 1; cur[4 * s.V] = nt; }
+                }
                 arr |= (uint64_t)g.ballot(arrives) << b0;
                 ndep += maro_popc(g.ballot(departs));
             }
@@ -1260,7 +1354,7 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
             g.sync();
             PHASE_MARK(r, PH_VESSELS);
             // ---- (b) events queued by earlier ticks
-            nev += run_bucket<G, kGeneral, kSmall>(s, g, r, tick);
+            if (!due) nev += run_bucket<G, kGeneral, kSmall>(s, g, r, tick);
             PHASE_MARK(r, PH_BUCKET);
             if (!kGeneral && (kSmall || s.DL)) nev += run_delay_line<G, kSmall>(s, g, r, tick);
             PHASE_MARK(r, PH_DELAY);
@@ -1285,7 +1379,7 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
             while (m) {
                 int v = maro_ffs64(m) - 1;
                 m &= m - 1;
-                run_arrival<G, kSmall>(s, g, r, tick, v);
+                run_arrival<G, kGeneral, kSmall>(s, g, r, tick, v);
                 nev += 2;
             }
             PHASE_MARK(r, PH_ARRIVALS);
@@ -1296,7 +1390,13 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
         uint64_t m = dec_pos >= 64 ? 0 : (arr >> dec_pos) << dec_pos;
         if (m) {
             int v = maro_ffs64(m) - 1;
-            take_snapshot(s, g, r, k, frame_index_of<kSmall>(s, tick));  // core.py:345
+            if (kDeferSnap) {  // core.py:345, written by flush_deferred_snapshot if it is ever observable
+                k.last_frame = frame_index_of<kSmall>(s, tick);
+                k.nsnaps += 1;
+                k.snap_pending = true;
+            } else {
+                take_snapshot(s, g, r, k, frame_index_of<kSmall>(s, tick));  // core.py:345
+            }
             if (g.lane == 0) {
                 int port = VA(s, r, VA_LOC_PORT_IDX, v);
                 int pe = PA(s, r, PA_EMPTY, port), sp = VA(s, r, VA_REMAINING_SPACE, v);
@@ -1370,7 +1470,8 @@ MARO_DEV void replica_step(const CimShape& s, const Grp<G>& g, const Replica& r,
     od[7] = k.ep_step;  // ordinal of this env-step inside the episode (0 = first decision)
     k.ep_step += 1;
     if (g.lane == 0) store_out(dec, met, od, bk, sh, k.opnum);
-    snapshot_wait(g);  // the pre-decision snapshot (if any) has been read: the caller may touch the frame again
+    if (kDeferSnap) g.sync();  // (no bulk read of the frame outstanding: the end-of-tick snapshots wait for theirs)
+    else snapshot_wait(g);     // the pre-decision snapshot (if any) has been read: the caller may touch the frame again
     PHASE_COUNT(r, PH_TICKS, nticks);
     PHASE_MARK(r, PH_STORE);
 }
@@ -1417,7 +1518,14 @@ MARO_DEV void replica_reset(const CimShape& s, const Grp<G>& g, const Replica& r
         r.c[C_FIXED + v] = dc;
         r.c[C_FIXED + s.V + v] = dc < ns ? TBL_I(r, s.t_stop_leave, sb + dc) : NO_TICK;
         r.c[C_FIXED + 2 * s.V + v] = NO_TICK;  // next_loc_idx == 0: no arrival until the first departure
+        if (s.due_R) {  // due rings: the first stop due at or after start_tick (nothing is outstanding before it)
+            int ds = 0;
+            while (ds < ns && TBL_I(r, s.t_stop_arrival, sb + ds) < s.start_tick) ds++;
+            r.c[C_FIXED + 3 * s.V + v] = ds;
+            r.c[C_FIXED + 4 * s.V + v] = ds < ns ? TBL_I(r, s.t_stop_arrival, sb + ds) : NO_TICK;
+        }
     }
+    LANE_LOOP(i, 2 * s.V * s.due_R) r.f[s.o_due + i] = 0;
     // queue: all slots on the free stack (slot 0 on top so that allocation order is ascending), empty buckets
     uint16_t* fs = q_free(s, r);
     uint16_t* nx = q_next(s, r);

@@ -299,7 +299,7 @@ __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __g
             }
             PHASE_MARK(r, PH_AGENT);
             PHASE_COUNT(r, PH_STEPS, 1);
-            replica_step<G, kGeneral, kSmall>(s, g, r, k, act, n_act, dslot, mslot);
+            replica_step<G, kGeneral, kSmall, true>(s, g, r, k, act, n_act, dslot, mslot);
             if (ra.trace && g.lane < 2)
                 reinterpret_cast<int4*>(ra.trace + ((int64_t)step * s.n_replicas + rep) * 8)[g.lane] = reinterpret_cast<const int4*>(dslot)[g.lane];
             const int status = dslot[MARO_DEC_STATUS];
@@ -313,6 +313,7 @@ __global__ void __launch_bounds__(256, kMinBlocks) cim_resident_kernel(const __g
             for (int i = 0; i < PH_SLOTS; i++) atomicAdd(&maro_phase_clk[i], pclk.acc[i]);
         r.pc = nullptr;
 #endif
+        flush_deferred_snapshot<G, kSmall>(s, g, r, k);  // (the work item ends: its last decision's snapshot becomes observable)
         if (ra.trace)
             for (; step < k_end; step++)
                 if (g.lane < 2)
@@ -1133,7 +1134,10 @@ int maro_cim_set_topology(MaroCimEnv* e, int32_t index, const MaroCimTopology* t
     {   // the handle's calendar-queue horizon, default queue capacity and RNG paths were sized from the create-time
         // topologies: a replacement has to fit them (an event beyond the horizon would alias into an earlier bucket)
         const CimTopoNeeds n = topology_needs(*topo);
-        if (n.max_delay + 1 > e->s.QH)
+        if (e->s.due_R && !n.stops_increase)  // (the due-ring drain takes one stop per vessel and tick)
+            return fail("maro_cim_set_topology: the new instance has a vessel whose stop ticks do not strictly increase; the handle "
+                        "keeps its discharges per stop (create the handle with this instance among its topologies)");
+        if (!e->s.due_R && n.max_delay + 1 > e->s.QH)
             return fail("maro_cim_set_topology: the new instance needs an event horizon of " + std::to_string(n.max_delay + 1) +
                         " ticks, the handle was created with " + std::to_string(e->s.QH) + " (create the handle with this instance among its topologies)");
         if ((n.order_noise && !e->s.order_noise) || (n.buffer_noise && !e->s.buffer_noise))

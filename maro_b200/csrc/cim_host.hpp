@@ -197,11 +197,18 @@ inline int check_same_shape(const MaroCimTopology& a, const MaroCimTopology& b) 
 // Fill `s` (layout, queue sizing) and serialise every topology into `tables`.  Returns non-zero on mismatch.
 // What one topology instance asks of a handle's sizing: the longest event delay (calendar-queue horizon), the buffer
 // ticks behind the default queue capacity, and which MT19937 streams it draws from.
-struct CimTopoNeeds { int max_delay = 2, buf_full = 1, buf_empty = 1, max_stops = 0; bool order_noise = false, buffer_noise = false; };
+// `stops_increase`: every vessel visits its stops at strictly increasing ticks (the condition of the due rings).
+struct CimTopoNeeds {
+    int max_delay = 2, buf_full = 1, buf_empty = 1, max_stops = 0;
+    bool order_noise = false, buffer_noise = false, stops_increase = true;
+};
 inline CimTopoNeeds topology_needs(const MaroCimTopology& t) {
     CimTopoNeeds n;
     const int P = t.n_ports, V = t.n_vessels;
     n.max_stops = t.stop_offset[V];
+    for (int v = 0; v < V; v++)
+        for (int i = t.stop_offset[v] + 1; i < t.stop_offset[v + 1]; i++)
+            if (t.stop_arrival[i] <= t.stop_arrival[i - 1]) n.stops_increase = false;
     for (int p = 0; p < P; p++) {
         if (t.source_noise[p] != 0) n.order_noise = true;
         if (t.full_return_noise[p] != 0 || t.empty_return_noise[p] != 0) n.buffer_noise = true;
@@ -241,10 +248,12 @@ inline int compute_shape_and_tables(const MaroCimTopology* topos, int n_topos, c
     s.DW = s.joint ? MARO_CIM_DECISION_WORDS * V : MARO_CIM_DECISION_WORDS;
     if (s.joint && s.max_actions < V) s.max_actions = V;  // one answer row per decision event of a tick
     int max_stops = 0, max_targets = t0.target_offset[P], max_delay = 2, max_rl = 1, buf_full = 1, buf_empty = 1;
+    bool stops_increase = true;
     for (int r = 0; r < t0.n_routes; r++) max_rl = std::max(max_rl, t0.route_offset[r + 1] - t0.route_offset[r]);
     s.max_route_len = max_rl;
     for (int k = 0; k < n_topos; k++) {
         const CimTopoNeeds n = topology_needs(topos[k]);
+        stops_increase = stops_increase && n.stops_increase;
         max_stops = std::max(max_stops, n.max_stops);
         if (n.order_noise) s.order_noise = 1;
         if (n.buffer_noise) s.buffer_noise = 1;
@@ -266,28 +275,42 @@ inline int compute_shape_and_tables(const MaroCimTopology* topos, int n_topos, c
     s.o_vp = s.o_fov + V * P;
     s.FW = s.o_vp + V * P;
     s.FWp = round_up(s.FW, 4);
-    s.CWp = round_up(C_FIXED + 3 * V, 4);
-    int qh = 16;
-    while (qh < max_delay + 1) qh <<= 1;
-    s.QH = qh;
-    // outstanding dynamic events: RETURN_FULL <= orders/tick x buffer, DISCHARGE_FULL <= V x route, RETURN_EMPTY
-    int qn = cfg->queue_capacity > 0 ? cfg->queue_capacity
-                                     : std::max(32, max_targets * buf_full + V * max_rl * (1 + buf_empty));
-    if (qn > 65000) qn = 65000;
-    s.QN = round_up(qn, 4);
-    s.SW = round_up(s.FWp + s.CWp + s.QN * 2 + s.QH + s.QN, 4);  // frame | ctrl | ev | buckets | next+free (u16)
     // delay lines for the pure-add events of noise-free, small topologies (cim_core.cuh: CimShape::DL): sized for the longest
     // container buffer time; the calendar queue then only carries DISCHARGE_FULL.  MARO_B200_DELAY_LINE=0 turns them off (A/B).
-    {
-        const bool noise_free = !s.order_noise && s.order_mode == 0 && !s.buffer_noise;
-        int dl = 2;
-        while (dl < std::max(buf_full, buf_empty) + 1) dl <<= 1;
-        const int stride = round_up(P * P + P + 2, 4);
-        const char* off = getenv("MARO_B200_DELAY_LINE");
-        if (noise_free && dl * stride <= 512 && !(off && atoi(off) == 0)) {
-            s.DL = dl; s.dl_stride = stride; s.o_dl = s.SW;  // (word offset from the start of the block = from r.f)
-            s.SW = round_up(s.SW + dl * stride, 4);
-        }
+    int dl = 2;
+    while (dl < std::max(buf_full, buf_empty) + 1) dl <<= 1;
+    const int dl_stride = round_up(P * P + P + 2, 4);
+    const char* dl_off = getenv("MARO_B200_DELAY_LINE");
+    const bool noise_free = !s.order_noise && s.order_mode == 0 && !s.buffer_noise;
+    const bool dl_on = noise_free && dl * dl_stride <= 512 && !(dl_off && atoi(dl_off) == 0);
+    // due rings for DISCHARGE_FULL where every vessel's stop ticks increase strictly (CimShape::due_R): the calendar queue is
+    // then not used at all and keeps no slots or buckets
+    if (dl_on && stops_increase) {
+        s.due_R = 1;
+        while (s.due_R < max_rl + 1) s.due_R <<= 1;
+    }
+    s.CWp = round_up(C_FIXED + (s.due_R ? 5 : 3) * V, 4);
+    if (s.due_R) {
+        s.QH = 0;
+        s.QN = 0;
+    } else {
+        int qh = 16;
+        while (qh < max_delay + 1) qh <<= 1;
+        s.QH = qh;
+        // outstanding dynamic events: RETURN_FULL <= orders/tick x buffer, DISCHARGE_FULL <= V x route, RETURN_EMPTY
+        int qn = cfg->queue_capacity > 0 ? cfg->queue_capacity
+                                         : std::max(32, max_targets * buf_full + V * max_rl * (1 + buf_empty));
+        if (qn > 65000) qn = 65000;
+        s.QN = round_up(qn, 4);
+    }
+    s.SW = round_up(s.FWp + s.CWp + s.QN * 2 + s.QH + s.QN, 4);  // frame | ctrl | ev | buckets | next+free (u16)
+    if (dl_on) {
+        s.DL = dl; s.dl_stride = dl_stride; s.o_dl = s.SW;  // (word offset from the start of the block = from r.f)
+        s.SW = round_up(s.SW + dl * dl_stride, 4);
+    }
+    if (s.due_R) {
+        s.o_due = s.SW;
+        s.SW = round_up(s.SW + 2 * V * s.due_R, 4);
     }
     s.res_is_one = s.resolution == 1 ? 1 : 0;
     s.vol_is_one = s.vol == 1.0 ? 1 : 0;
@@ -325,9 +348,9 @@ inline int lanes_per_replica(const CimShape& s) {
 
 // May replica_step<G, false, kSmall = true> run this shape with G lanes per replica?  Noise-free fixed-order mode with
 // integer buffer ticks (the kGeneral = false path), snapshot resolution 1, container volume 1, Sequential mode, delay
-// lines on, and every dimension a lane loop runs over (ports, vessels, route stops, future stops) <= G.
+// lines and due rings on, and every dimension a lane loop runs over (ports, vessels, route stops, future stops) <= G.
 inline bool cim_small_ok(const CimShape& s, int G) {
-    return s.order_table && !s.order_noise && !s.buffer_noise && s.res_is_one && s.vol_is_one && !s.joint && s.DL > 0 &&
+    return s.order_table && !s.order_noise && !s.buffer_noise && s.res_is_one && s.vol_is_one && !s.joint && s.DL > 0 && s.due_R > 0 &&
            s.P <= G && s.V <= G && s.max_route_len <= G && s.fut <= G;
 }
 

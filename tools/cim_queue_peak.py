@@ -2,6 +2,8 @@
 
 The device code is compiled for the host with -DMARO_TRACK_QPEAK (tests/_emul_src/emul.cpp, thread-per-lane emulator) and an
 episode is played per seed with a random agent.  Build container only; used to size `queue_capacity` head-room claims in DESIGN.md.
+Noise-free handles with delay lines and due rings (toy.*_l0.0: every vessel's stop ticks increase strictly) do not use the
+queue at all (`QN = 0`): their peak is 0 and `queue_capacity` does not apply to them.
 
     python tools/cim_queue_peak.py global_trade.22p_l0.8 500 4096 4097 4098
 """
