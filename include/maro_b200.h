@@ -175,7 +175,8 @@ int maro_cim_step_device(MaroCimEnv* env, const uint8_t* d_active, const int32_t
 /* Env.reset (core.py:143-170) for the replicas selected by mask (NULL = all).  Tables of the replicas'
  * topologies must already be resident (see maro_cim_set_topology for keep_seed=False / set_seed).  While the resident
  * kernel is live the reset costs nothing here: it rides on each replica's next command row and is carried out in shared
- * memory (any call that reads device state applies what is still pending first). */
+ * memory (any call that reads device state applies what is still pending first).  The mask is read during the call; no
+ * pinned staging buffer (maro_cim_pinned_buffers) is written, so inputs filled there for the next step survive a reset. */
 int maro_cim_reset(MaroCimEnv* env, const uint8_t* mask);
 /* Replace topology slot `index` (same shape) — used for reset(keep_seed=False) and Env.set_seed. */
 int maro_cim_set_topology(MaroCimEnv* env, int32_t index, const MaroCimTopology* topo);
@@ -358,6 +359,8 @@ int maro_bike_step_device(MaroBikeEnv* env, const uint8_t* d_active, const int32
 /* Fused rollout (like maro_cim_rollout_device): n_steps env-steps per replica in one launch with the greedy top-1 agent of
  * examples/citi_bike/greedy/launcher.py:35-65 as a device callback; d_decisions is in/out; a replica stops at its DONE row. */
 int maro_bike_rollout_device(MaroBikeEnv* env, int32_t n_steps, int32_t* d_decisions, int64_t* d_metrics);
+/* Env.reset for the replicas selected by mask (NULL = all).  The mask is read during the call; no pinned staging buffer is
+ * written. */
 int maro_bike_reset(MaroBikeEnv* env, const uint8_t* mask);
 /* Per-replica seeds of the transfer_time stream: the reference draws `round(np.random.normal(mean, std))` per action
  * (citi_bike/decision_strategy.py:213-216) from the process-global numpy RandomState, and every env of a VectorEnv is its
@@ -460,6 +463,8 @@ int maro_vm_step_device(MaroVmEnv* env, const uint8_t* d_active, const int32_t* 
 int maro_vm_pinned_buffers(MaroVmEnv* env, void** actions, void** n_actions, void** active, void** decisions,
                            void** metrics);
 int maro_vm_step_pinned(MaroVmEnv* env, int32_t use_actions, int32_t use_n_actions, int32_t use_active);
+/* Env.reset for the replicas selected by mask (NULL = all).  The mask is read during the call; no pinned staging buffer is
+ * written. */
 int maro_vm_reset(MaroVmEnv* env, const uint8_t* mask);
 int maro_vm_query(MaroVmEnv* env, const int32_t* replicas, int32_t n_replicas, int32_t node_type,
                   const int32_t* frame_indices, int32_t n_frames, const int32_t* nodes, int32_t n_nodes,

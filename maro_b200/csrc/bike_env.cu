@@ -206,12 +206,7 @@ int maro_bike_reset(MaroBikeEnv* e, const uint8_t* mask) {
     if (!e) return fail("null handle");
     CK(cudaSetDevice(e->device));
     BikeArgs a = bike_base_args(e);
-    if (mask) {
-        uint8_t* d_active = e->d_in + (size_t)e->B * e->max_actions * 16 + (size_t)e->B * 4;
-        memcpy(e->h_in, mask, e->B);
-        CK(cudaMemcpyAsync(d_active, e->h_in, e->B, cudaMemcpyHostToDevice, e->stream));
-        a.active = d_active;
-    }
+    if (mask && common_stage_mask(e, mask, &a.active)) return 1;
     int threads = 128, blocks = std::min((e->B * 32 + threads - 1) / threads, e->n_sm * 16);
     bike_reset_kernel<<<blocks, threads, 0, e->stream>>>(e->s, a);
     CK(cudaGetLastError());

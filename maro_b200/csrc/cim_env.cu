@@ -1103,12 +1103,8 @@ int maro_cim_reset(MaroCimEnv* e, const uint8_t* mask) {
 
 static int reset_now(MaroCimEnv* e, const uint8_t* mask) {
     StepArgs a = base_args(e);
-    if (mask) {  // staged through the pinned `active` region (never through the caller-visible action rows)
-        const size_t active_off = (size_t)e->B * e->s.max_actions * 16 + (size_t)e->B * 4;
-        uint8_t* d_active = e->d_in + active_off;
-        if (mask != e->h_in + active_off) memcpy(e->h_in + active_off, mask, e->B);
-        CK(cudaMemcpyAsync(d_active, e->h_in + active_off, e->B, cudaMemcpyHostToDevice, e->stream));
-        a.active = d_active;
+    if (mask) {
+        if (common_stage_mask(e, mask, &a.active)) return 1;
         for (int i = 0; i < e->B; i++) if (mask[i]) e->reset_pending[i] = 0;
     } else {
         std::fill(e->reset_pending.begin(), e->reset_pending.end(), (uint8_t)0);

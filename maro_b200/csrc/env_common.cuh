@@ -167,6 +167,11 @@ static int common_alloc(EnvCommon* e) {
     CK(cudaMalloc(&e->d_state, B * e->SW * 4));
     CK(cudaMalloc(&e->d_snap, B * e->ring_rows * e->FWp * 4));
     CK(cudaMalloc(&e->d_snap_frame, B * e->ring_rows * 4));
+    // cudaMalloc may hand back memory a freed handle of this process used.  The work counters of the state blocks persist
+    // across resets (no reset writes them), so the blocks start from zeros; the ring starts empty.
+    CK(cudaMemset(e->d_state, 0, B * e->SW * 4));
+    CK(cudaMemset(e->d_snap, 0, B * e->ring_rows * e->FWp * 4));
+    CK(cudaMemset(e->d_snap_frame, 0xff, B * e->ring_rows * 4));
     e->in_bytes = B * e->max_actions * 16 + B * 4 + round_up(e->B, 16);
     e->out_bytes = B * e->dec_words * 4 + B * e->met_words * 8;
     CK(cudaMalloc(&e->d_in, e->in_bytes));
@@ -220,7 +225,19 @@ static int common_host_step(EnvCommon* e, const uint8_t* active, const int32_t* 
     return 0;
 }
 
-static int common_pinned_buffers(EnvCommon* e, void** actions, void** n_actions, void** active, void** decisions, void** metrics) {
+// Reset masks go straight from the caller's bytes into the device-side active region of d_in.  The pinned staging buffers
+// belong to the caller between steps (actions / n_actions / active filled for the next step_pinned, or read by a submit on
+// another replica range), so a reset must not write them.  d_in's active region is private to the library: the bulk-copy
+// step refills it before every use and the zero-copy step reads hd_in.  The caller synchronises the stream before
+// returning, so a pageable mask is fine.
+static int common_stage_mask(EnvCommon* e, const uint8_t* mask, const uint8_t** d_active) {
+    uint8_t* dst = e->d_in + (size_t)e->B * e->max_actions * 16 + (size_t)e->B * 4;
+    CK(cudaMemcpyAsync(dst, mask, e->B, cudaMemcpyHostToDevice, e->stream));
+    *d_active = dst;
+    return 0;
+}
+
+static int common_pinned_buffers(EnvCommon* e,void** actions, void** n_actions, void** active, void** decisions, void** metrics) {
     if (!e) return fail("pinned_buffers: null handle");
     const size_t B = (size_t)e->B, act_bytes = B * e->max_actions * 16;
     if (actions) *actions = e->h_in;

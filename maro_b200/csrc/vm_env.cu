@@ -178,12 +178,7 @@ static int vm_reset_impl(MaroVmEnv* e, const uint8_t* mask, int init_ring) {
     if (!e) return fail("null handle");
     CK(cudaSetDevice(e->device));
     VmArgs a = vm_base_args(e);
-    if (mask) {
-        uint8_t* d_active = e->d_in + (size_t)e->B * e->max_actions * 16 + (size_t)e->B * 4;
-        memcpy(e->h_in, mask, e->B);
-        CK(cudaMemcpyAsync(d_active, e->h_in, e->B, cudaMemcpyHostToDevice, e->stream));
-        a.active = d_active;
-    }
+    if (mask && common_stage_mask(e, mask, &a.active)) return 1;
     int threads = 128, blocks = std::min((e->B * 32 + threads - 1) / threads, e->n_sm * 16);
     vm_reset_kernel<<<blocks, threads, 0, e->stream>>>(e->s, a, init_ring);
     CK(cudaGetLastError());
